@@ -19,19 +19,23 @@ Printed JSON (one line, rank 0):
              H2D + compute + D2H of the pooled rows inside the timed region; at N > 1 the all-gather of
              the ranks' result matrices is inside it too
   roofline   tensor-core bound: the dominant kernel (FFN-up GEMM) timed alone with CUDA events against
-             the measured burst bf16 peak, its DRAM traffic per launch from the committed ncu capture
-             (profiles/ncu_traffic.json), and under "whole_step" the step-level achieved TFLOP/s
-             (algorithmic matmul FLOPs, SURVEY 8d) against the measured sustained bf16 peak
-  cpu_baseline  the UNMODIFIED reference (baseline/_ref: `distllm.distributed_embedding.embedding_worker`,
+             the dense 16-bit tensor peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet),
+             and under "whole_step" the step-level achieved TFLOP/s (algorithmic matmul FLOPs, SURVEY 8d)
+             against the same peak
+  cpu_baseline  the UNMODIFIED reference (oracle/_ref: `distllm.distributed_embedding.embedding_worker`,
              its own `[timer] [computed-embeddings ...]` reading) on this box's host cores on a bounded
              sample, in a CPU-only subprocess (rank 0, N=1 only); plus the cosine between its embeddings
              and this repository's for the same checkpoint and file.  Falls back to the oracle port
-             (kind "port") when baseline/_ref is absent.
+             (kind "port") when oracle/_ref is absent.
   extra      the other BASELINE configs and the plugin-level numbers, each with its own roofline fraction:
              ragged (lengths ~U{64..512}), c5_esm2_650m (S=1026), c3_mistral7b (B=16, S=4096),
              c4_gather (N > 1: >= 2 M rows per rank through the all-gather), e2e_worker (tokeniser ->
              embedding_worker -> writer), c1 (1 000 x 128-token chunks, batch 8, through the worker)
 --impl reference times the unmodified reference as its own arm (rank 0 only; CUDA hidden from it).
+--dump-outputs DIR writes what the last timed step computed, as rank 0 holds it after the all-gather: the
+pooled rows of every rank's last batch (rank order) and their adjacent cosine distances, as float32 .npy files
+(1.5 MB + 2 KB per GPU).  Inputs and weights are seeded, so two builds of the
+project run on the same arguments can be compared output for output.
 """
 
 from __future__ import annotations
@@ -65,7 +69,8 @@ BERT_BASE = workloads.BERT_BASE
 WORKLOAD = ('C2: S-PubMedBert-MS-MARCO shape (BERT-base L12 H768 I3072), mean pooler (reference '
             'semantics), batch_size=512, 512-token chunks, pre-tokenised synthetic ids, random-init weights')
 METRIC = 'embedded chunks/sec @512-tok'
-FALLBACK_PEAKS = {'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0, 'hbm_gbs': 6650.0}
+# H100 SXM data sheet (700 W): dense BF16 / FP16 tensor rate and HBM3 bandwidth; never reached in practice
+FALLBACK_PEAKS = {'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0, 'hbm_gbs': 3350.0}
 ESM2_650M = dict(vocab_size=33, hidden_size=1280, num_hidden_layers=33, num_attention_heads=20,
                  intermediate_size=5120, max_position_embeddings=1026, position_embedding_type='rotary',
                  token_dropout=True, mask_token_id=32, pad_token_id=1, layer_norm_eps=1e-5,
@@ -94,8 +99,7 @@ def mistral_flops_per_seq(cfg: dict, s: int, causal_skipped: bool = True) -> flo
 def launches_per_step(cfg: dict) -> int:
     """Kernels of ours per step: the 3 kernels of the padding-free layout (lengths, scan, row map), embed+LN,
     attention mask prep, per layer 4 GEMMs + attention + 2 LayerNorms (the last LayerNorm is the fused LN+pool),
-    3 pool-weight kernels, pool finalize, adjacent-cosine (matches profiles/r02_ncu_launches_final.md: 1413
-    launches in 15 passes)."""
+    3 pool-weight kernels, pool finalize, adjacent-cosine."""
     return 3 + 1 + 1 + cfg['num_hidden_layers'] * 7 + 3 + 1 + 1
 
 
@@ -124,7 +128,7 @@ def synthetic_batch(n: int, s: int, vocab: int, seed: int, ragged: tuple[int, in
 
 
 class ClockSampler:
-    """nvidia-smi clock/throttle sampling during the timed region (recipe in B200_PROFILING.md)."""
+    """nvidia-smi clock/throttle sampling during the timed region (read-only queries)."""
 
     QUERY = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,'
              'clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
@@ -291,7 +295,7 @@ _CPU_WEIGHTS: dict = {}
 
 
 def cpu_oracle_run(n_chunks: int, batch: int, seed: int = 0):
-    """FALLBACK when baseline/_ref is absent: time the CPU port of the reference path (oracle forward +
+    """FALLBACK when oracle/_ref is absent: time the CPU port of the reference path (oracle forward +
     reference mean pool) on ``n_chunks`` synthetic 512-token chunks.  Returns (seconds, chunks)."""
     from transformers import BertConfig
 
@@ -327,7 +331,7 @@ def run_reference_port(args) -> None:
         'config': {'workload': WORKLOAD, 'global_batch': 8, 'seq_len': SEQ, 'parallelism': 'cpu',
                    'sample_chunks_per_step': per_step},
         'cpu_baseline': {'value': value, 'unit': 'chunks/s', 'cores': threads, 'kind': 'port', 'sample': sample,
-                         'note': 'baseline/_ref absent: the oracle port ran instead of the reference'},
+                         'note': 'oracle/_ref absent: the oracle port ran instead of the reference'},
         'e2e': {'value': value, 'unit': 'chunks/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
         'gpu_launches': 0,
     }, args.json_out)
@@ -387,16 +391,7 @@ def storage_ab(device: torch.device) -> dict:
     return out
 
 
-DOMINANT_KERNEL = 'gemm2_h16_pair<5,GELU> (FFN up, M=262144 N=3072 K=768; CTA-pair tcgen05 kernel, bfloat16 build)'
-
-
-def ncu_traffic_bytes() -> float | None:
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the
-    committed `ncu --set full` summary (profiles/ncu_traffic.json, written by tools/ncu_traffic.py)."""
-    path = REPO / 'profiles' / 'ncu_traffic.json'
-    if not path.exists():
-        return None
-    return json.loads(path.read_text()).get('ffn_up_gemm_b512', {}).get('dram_bytes_per_launch')
+DOMINANT_KERNEL = 'gemm_h16_wgmma<GELU> (FFN up, M=262144 N=3072 K=768; bfloat16 build)'
 
 
 def timed_steps(fn, steps: int, warm: int, device) -> float:
@@ -581,7 +576,7 @@ def cpu_baseline_leg(device) -> dict:
             sec, n = cpu_oracle_run(n_chunks, 8)
             return {'value': n / sec, 'unit': 'chunks/s', 'cores': torch.get_num_threads(), 'kind': 'port',
                     'sample': f'{n} chunks of {SEQ} tokens, batch 8, fp32 torch CPU oracle ({sec:.1f} s); '
-                              'baseline/_ref absent'}
+                              'oracle/_ref absent'}
         ckpt = workloads.write_bert_checkpoint(tmp / 'ckpt')
         sample = workloads.write_token_rows(tmp / 'sample.jsonl', n_chunks, SEQ, BERT_BASE['vocab_size'], seed=123)
         cmd = [sys.executable, str(REPO / 'bench.py'), '--impl', 'reference', '--steps', '1', '--warmup', '0',
@@ -625,7 +620,7 @@ def run_native(args) -> None:
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
     partition_host_threads()   # each rank its share of the host cores (the product's torchrun driver does the same)
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py --impl native needs a B200; there is no CPU fallback')
+        raise SystemExit('bench.py --impl native needs an H100; there is no CPU fallback')
     build_native()
     torch.cuda.set_device(local_rank)
     device = torch.device('cuda', local_rank)
@@ -687,6 +682,18 @@ def run_native(args) -> None:
     elapsed_s = reduce_max(e0.elapsed_time(e1)) * 1e-3
     clocks = sampler.stop() if rank == 0 else None
     assert gathered.shape[0] == world * steps * BATCH
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        # what the caller holds after the last step: every rank's batch of it from the gathered matrix (rank
+        # order), and the adjacent-cosine distances each rank computed on its batch (the same kernel on the
+        # same rows, so recomputing them here gives the timed step's values)
+        last = [gathered[(r * steps + steps - 1) * BATCH:(r * steps + steps) * BATCH] for r in range(world)]
+        dump = Path(args.dump_outputs)
+        dump.mkdir(parents=True, exist_ok=True)
+        np.save(dump / 'pooled.npy', torch.cat(last).float().cpu().numpy())
+        np.save(dump / 'adjacent_cosine_dist.npy',
+                torch.cat([nv.adjacent_cosine_dist(x) for x in last]).float().cpu().numpy())
     del gathered
     value = world * steps * BATCH / elapsed_s
 
@@ -767,13 +774,13 @@ def run_native(args) -> None:
         # top level: the dominant kernel against the burst peak (timed alone); whole_step: all 94
         # launches of one step against the sustained peak
         roof = {'bound': 'tensor', 'achieved': dom['achieved'], 'peak': dom['peak'], 'unit': 'TFLOP/s',
-                'frac': dom['frac'], 'traffic': ncu_traffic_bytes(), 'kernel': dom['name'],
+                'frac': dom['frac'], 'kernel': dom['name'],
                 'flops_per_launch': dom['flops_per_launch'], 'ms_per_launch': dom['ms_per_launch'],
-                'peak_source': f'{peak_src} burst 16-bit (bf16 cuBLAS) tensor peak (kernel timed alone)',
+                'peak_source': f'{peak_src} dense 16-bit tensor peak (kernel timed alone)',
                 'whole_step': {'achieved': step_tf, 'peak': peaks['bf16_tflops_sustained'],
                                'frac': step_tf / peaks['bf16_tflops_sustained'], 'unit': 'TFLOP/s',
                                'flops_per_chunk': fpc,
-                               'peak_source': f'{peak_src} sustained 16-bit (bf16 cuBLAS) tensor peak (whole step, per GPU)'}}
+                               'peak_source': f'{peak_src} dense 16-bit tensor peak (whole step, per GPU)'}}
         cpu_base = None
         if world == 1 and not args.no_cpu_baseline:
             cpu_base = cpu_baseline_leg(device)
@@ -783,7 +790,7 @@ def run_native(args) -> None:
             'scaling': 'weak', 'vs_baseline': None, 'dtype': enc_storage, 'data': 'synthetic',
             'config': {'workload': WORKLOAD, 'global_batch': BATCH * world, 'seq_len': SEQ,
                        'parallelism': f'dp{world}: chunks sharded by rank, one all-gather of the pooled matrix',
-                       'l2': 'per-step activations (~4 GB) exceed the 126 MB L2; no explicit flush needed'},
+                       'l2': 'per-step activations (~4 GB) exceed the 50 MB L2; no explicit flush needed'},
             'e2e': {'value': e2e_value, 'unit': 'chunks/s', 'h2d_bytes_per_step': 3 * BATCH * SEQ * 8,
                     'd2h_bytes_per_step': BATCH * hidden * 4, 'steps': e2e_steps,
                     'api': 'b2e_embed_host (C ABI, pinned host buffers)' + (
@@ -814,6 +821,9 @@ def main() -> None:
     ap.add_argument('--json-out', default=None, help='also write the JSON line to this file')
     ap.add_argument('--embeddings-out', default=None, help='copy the last step embeddings.npy here')
     ap.add_argument('--no-c1', dest='with_c1', action='store_false', help='skip the C1 (1000 x 128-token) run')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help="write the last timed step's pooled rows of every rank (from the gathered matrix) and their "
+                         "adjacent cosine distances as DIR/<name>.npy")
     args = ap.parse_args()
     # stdout carries exactly one JSON line: everything libraries write to fd 1 while the benchmark
     # runs (NCCL's version banner, progress bars) is sent to stderr; emit() writes to the saved fd

@@ -1,4 +1,4 @@
-"""distllm_b200: B200-native (sm_100a) implementation of distllm's embedding hot path."""
+"""distllm_b200: H100-native (sm_90a) implementation of distllm's embedding hot path."""
 
 from __future__ import annotations
 

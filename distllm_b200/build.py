@@ -1,4 +1,4 @@
-"""In-tree build of the native library (libb2e.so) with nvcc for sm_100a.
+"""In-tree build of the native library (libb2e.so) with nvcc for sm_90a.
 
 nvcc cross-compiles without a GPU, so this runs on the authoring box too; the built .so sits next
 to the package (git-ignored) and travels with the tree.
@@ -24,7 +24,7 @@ NVCC_FLAGS = [
     '-O3',
     '-std=c++17',
     '-gencode',
-    'arch=compute_100a,code=sm_100a',
+    'arch=compute_90a,code=sm_90a',
     '-lineinfo',
     '-Xcompiler',
     '-fPIC',

@@ -1,5 +1,5 @@
-// libb2e.so -- C ABI (include/b2e.h) over the sm_100a kernels.  Host runtime only: handle,
-// lazily grown workspace, TMA descriptors and launches.  No CPU fallback: without an sm_100 device
+// libb2e.so -- C ABI (include/b2e.h) over the sm_90a kernels.  Host runtime only: handle,
+// lazily grown workspace, TMA descriptors and launches.  No CPU fallback: without an sm_90 device
 // every compute entry point fails with B2E_ERR_NO_DEVICE.
 #include "../../include/b2e.h"
 #include "../../include/b2e_debug.h"
@@ -15,13 +15,10 @@
 #include <utility>
 #include <vector>
 
-#include "attention3.cuh"
-#include "attention4.cuh"
-#include "attention5.cuh"
+#include "attention.cuh"
 #include "binsearch.cuh"
 #include "common.cuh"
 #include "gemm.cuh"
-#include "gemm2.cuh"
 #include "mistral_ops.cuh"
 #include "pack.cuh"
 #include "rowops.cuh"
@@ -130,8 +127,8 @@ int device_info(int device, DeviceInfo* info) {
   if (device < 0 || device >= n) return fail(B2E_ERR_INVALID, "device %d out of range", device);
   cudaDeviceProp p;
   CUDA_TRY(cudaGetDeviceProperties(&p, device));
-  if (p.major != 10)
-    return fail(B2E_ERR_NO_DEVICE, "device %d is sm_%d%d; libb2e is built for sm_100a only", device,
+  if (p.major != 9 || p.minor != 0)
+    return fail(B2E_ERR_NO_DEVICE, "device %d is sm_%d%d; libb2e is built for sm_90a only", device,
                 p.major, p.minor);
   info->sms = p.multiProcessorCount;
   info->cc_major = p.major;
@@ -172,83 +169,6 @@ int ensure_smem_attr(Kern kern, int bytes) {
 }
 
 // ---------------------------------------------------------------- launches
-template <int BN, int STAGES, int EPI>
-int launch_gemm_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
-                    const float* bias, const h16* resid, int M, int N, int K, int sms,
-                    cudaStream_t st, const int* m_dev = nullptr) {
-  using Cfg = GemmCfg<BN, STAGES>;
-  auto kern = gemm_h16_tcgen05_kernel<BN, STAGES, EPI>;
-  {
-    const int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES);
-    if (arc) return arc;
-  }
-  const int tiles = ((M + GEMM_BM - 1) / GEMM_BM) * (N / BN);
-  const int grid = tiles < sms ? tiles : sms;
-  static int cluster_probe = -1;  // B2E_GEMM=v1cluster: same kernel, launched as clusters of 2 (experiment)
-  if (cluster_probe < 0) {
-    const char* e = getenv("B2E_GEMM");
-    cluster_probe = (e && strcmp(e, "v1cluster") == 0) ? 1 : 0;
-  }
-  if (cluster_probe) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid & ~1);
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2;
-    at[0].val.clusterDim.y = 1;
-    at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ta, tb, tout, bias, resid, M, N, K, m_dev));
-    return B2E_OK;
-  }
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(ta, tb, tout, bias, resid, M, N, K, m_dev);
-  CUDA_TRY(cudaGetLastError());
-  return B2E_OK;
-}
-
-template <int BN, int STAGES>
-int launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
-                   const float* bias, const h16* resid, int M, int N, int K, int epi, int sms,
-                   cudaStream_t st, const int* m_dev = nullptr) {
-  switch (epi) {
-    case B2E_EPI_BIAS:
-      return launch_gemm_cfg<BN, STAGES, EPI_BIAS>(ta, tb, tout, bias, resid, M, N, K, sms, st, m_dev);
-    case B2E_EPI_BIAS_GELU:
-      return launch_gemm_cfg<BN, STAGES, EPI_BIAS_GELU>(ta, tb, tout, bias, resid, M, N, K, sms, st, m_dev);
-    case B2E_EPI_BIAS_RESID:
-      return launch_gemm_cfg<BN, STAGES, EPI_BIAS_RESID>(ta, tb, tout, bias, resid, M, N, K, sms,
-                                                         st);
-    case B2E_EPI_SWIGLU:
-      if constexpr (BN == 256)
-        return launch_gemm_cfg<256, STAGES, EPI_SWIGLU>(ta, tb, tout, bias, resid, M, N, K, sms, st, m_dev);
-      else
-        return fail(B2E_ERR_INVALID, "SwiGLU epilogue needs N %% 256 == 0");
-    case B2E_EPI_GEGLU:
-      if constexpr (BN == 256)
-        return launch_gemm_cfg<256, STAGES, EPI_GEGLU>(ta, tb, tout, bias, resid, M, N, K, sms, st, m_dev);
-      else
-        return fail(B2E_ERR_INVALID, "GeGLU epilogue needs N %% 256 == 0");
-  }
-  return fail(B2E_ERR_INVALID, "unknown epilogue %d", epi);
-}
-
-// The CTA-pair kernel (gemm2.cuh, 256 x 256 tiles over two SMs) is the default whenever N is a multiple
-// of 256; B2E_GEMM=single forces the single-CTA kernel (gemm.cuh), which also serves N % 256 == 128.
-inline bool gemm_use_pair() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("B2E_GEMM");
-    v = (e && strcmp(e, "single") == 0) ? 0 : 1;
-  }
-  return v == 1;
-}
-// rows of the W tile one TMA box covers: the pair kernel stages half of the 256-row tile per CTA
-inline int gemm_bn_for(int N) { return (N % 256 == 0 && !gemm_use_pair()) ? 256 : 128; }
-
 int check_gemm_shape(int M, int N, int K) {
   if (M <= 0 || N <= 0 || K <= 0) return fail(B2E_ERR_INVALID, "gemm: empty shape %dx%dx%d", M, N, K);
   if (N % 128 != 0) return fail(B2E_ERR_INVALID, "gemm: N=%d must be a multiple of 128", N);
@@ -256,61 +176,36 @@ int check_gemm_shape(int M, int N, int K) {
   return B2E_OK;
 }
 
-bool g_gemm2_profiling = false;   // b2e_debug_set_clock_buffer / b2e_debug_set_pair_flags: use the instrumented GEMM
+bool g_gemm_profiling = false;   // b2e_debug_set_clock_buffer: the bias GEMM runs its timeline instantiation
 
-template <int STAGES, int EPI>
-int launch_gemm2_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
-                     const float* bias, const h16* resid, int M, int N, int K, int sms,
-                     cudaStream_t st, const int* m_dev = nullptr) {
-  using Cfg = Gemm2Cfg<STAGES>;
-  const int tiles = ((M + 255) / 256) * (N / G2_BN);
-  int grid = 2 * tiles;
-  if (grid > (sms & ~1)) grid = sms & ~1;
-  if constexpr (EPI == EPI_BIAS) {
-    if (g_gemm2_profiling) {   // a clock buffer or an experiment flag is set: the instrumented instantiation
-      auto kern_tl = gemm2_h16_pair_kernel<STAGES, EPI, true>;
-      const int arc = ensure_smem_attr(kern_tl, Cfg::SMEM_BYTES);
-      if (arc) return arc;
-      kern_tl<<<grid, G2_THREADS, Cfg::SMEM_BYTES, st>>>(ta, tb, tout, bias, resid, M, N, K, m_dev);
-      CUDA_TRY(cudaGetLastError());
-      return B2E_OK;
-    }
-  }
-  auto kern = gemm2_h16_pair_kernel<STAGES, EPI>;
-  {
-    const int arc = ensure_smem_attr(kern, Cfg::SMEM_BYTES);
-    if (arc) return arc;
-  }
-  kern<<<grid, G2_THREADS, Cfg::SMEM_BYTES, st>>>(ta, tb, tout, bias, resid, M, N, K, m_dev);
+template <int EPI>
+int launch_gemm_epi(const CUtensorMap& ta, const CUtensorMap& tb, void* out, const float* bias,
+                    const h16* resid, int M, int N, int K, cudaStream_t st, const int* m_dev) {
+  auto kern = gemm_h16_wgmma_kernel<EPI>;
+  if constexpr (EPI == EPI_BIAS)
+    if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true>;
+  const int arc = ensure_smem_attr(kern, GEMM_SMEM_BYTES);
+  if (arc) return arc;
+  const long long tiles = (long long)(N / GEMM_BN) * ((M + GEMM_BM - 1) / GEMM_BM);
+  if (tiles > 0x7fffffffLL) return fail(B2E_ERR_INVALID, "gemm: %lld output tiles exceed one grid", tiles);
+  kern<<<(unsigned)tiles, GEMM_THREADS, GEMM_SMEM_BYTES, st>>>(ta, tb, static_cast<h16*>(out), bias, resid, M, N, K, m_dev);
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
 }
 
-// A map: [M,K] box 128 rows; W map: [N,K] box gemm_bn_for(N) rows.
+// A map: [M,K] box 128 rows; W map: [N,K] box GEMM_BN rows.
 // m_dev (nullable): device-resident row count <= M (packed token layout); M sizes the grid and the tensor maps.
 int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* out, const float* bias,
-                const void* resid, int M, int N, int K, int epi, int sms, cudaStream_t st,
-                const int* m_dev = nullptr) {
+                const void* resid, int M, int N, int K, int epi, cudaStream_t st, const int* m_dev = nullptr) {
   const h16* r = static_cast<const h16*>(resid);
-  // output tiles leave through TMA stores: [M,N] row-major, box = 64 columns x 32 rows
-  CUtensorMap tout;
-  int rc;
-  const bool glu = epi == B2E_EPI_SWIGLU || epi == B2E_EPI_GEGLU;
-  const int n_out = glu ? N / 2 : N;   // the gated epilogues write act(first) * second: [M, N/2]
-  if ((rc = make_tmap_h16(&tout, out, M, n_out, GEMM_OUT_BOX_ROWS))) return rc;
-  if (N % 256 == 0 && gemm_use_pair()) {
-    constexpr int PS = 5;   // 5 x 32 KiB stages + two staging tiles per epilogue warp
-    switch (epi) {
-      case B2E_EPI_BIAS: return launch_gemm2_cfg<PS, EPI_BIAS>(ta, tb, tout, bias, r, M, N, K, sms, st, m_dev);
-      case B2E_EPI_BIAS_GELU: return launch_gemm2_cfg<PS, EPI_BIAS_GELU>(ta, tb, tout, bias, r, M, N, K, sms, st, m_dev);
-      case B2E_EPI_BIAS_RESID: return launch_gemm2_cfg<PS, EPI_BIAS_RESID>(ta, tb, tout, bias, r, M, N, K, sms, st, m_dev);
-      case B2E_EPI_SWIGLU: return launch_gemm2_cfg<PS, EPI_SWIGLU>(ta, tb, tout, bias, r, M, N, K, sms, st, m_dev);
-      case B2E_EPI_GEGLU: return launch_gemm2_cfg<PS, EPI_GEGLU>(ta, tb, tout, bias, r, M, N, K, sms, st, m_dev);
-    }
-    return fail(B2E_ERR_INVALID, "unknown epilogue %d", epi);
+  switch (epi) {
+    case B2E_EPI_BIAS: return launch_gemm_epi<EPI_BIAS>(ta, tb, out, bias, r, M, N, K, st, m_dev);
+    case B2E_EPI_BIAS_GELU: return launch_gemm_epi<EPI_BIAS_GELU>(ta, tb, out, bias, r, M, N, K, st, m_dev);
+    case B2E_EPI_BIAS_RESID: return launch_gemm_epi<EPI_BIAS_RESID>(ta, tb, out, bias, r, M, N, K, st, m_dev);
+    case B2E_EPI_SWIGLU: return launch_gemm_epi<EPI_SWIGLU>(ta, tb, out, bias, r, M, N, K, st, m_dev);
+    case B2E_EPI_GEGLU: return launch_gemm_epi<EPI_GEGLU>(ta, tb, out, bias, r, M, N, K, st, m_dev);
   }
-  if (N % 256 == 0) return launch_gemm_bn<256, 4>(ta, tb, tout, bias, r, M, N, K, epi, sms, st, m_dev);
-  return launch_gemm_bn<128, 6>(ta, tb, tout, bias, r, M, N, K, epi, sms, st, m_dev);
+  return fail(B2E_ERR_INVALID, "unknown epilogue %d", epi);
 }
 
 // Per-forward attention inputs derived from the mask (attention3.cuh): additive key bias rows and
@@ -356,7 +251,7 @@ struct AttnScratch {
   }
 };
 
-inline int attn_s_pad(int S) { return (S + AT3_KC - 1) / AT3_KC * AT3_KC; }
+inline int attn_s_pad(int S) { return (S + AT_KC - 1) / AT_KC * AT_KC; }
 
 int attention_prepare(AttnScratch& sc, const int64_t* mask, int B, int S, cudaStream_t st) {
   int rc;
@@ -367,21 +262,6 @@ int attention_prepare(AttnScratch& sc, const int64_t* mask, int B, int S, cudaSt
   return B2E_OK;
 }
 
-// Softmax variant of the head_dim-64 attention kernel (template parameter V of attention3_d64_kernel);
-// B2E_ATT3=<n> or b2e_debug_set_att3_variant picks one of the instantiated ones for A/B measurements.
-// 65 = four softmax warpgroups (attention5.cuh), fully attended chunks known from attn_prep: same-box A/B of the whole
-// step against 5 (two warpgroups + one exponential in four on the FMA pipe): C2 49.58 vs 49.81 ms, C5 100.6 vs 102.5 ms
-// (profiles/r02_step_ab_att5.log); both kernels pass the same tests.
-constexpr int AT3_DEFAULT_VARIANT = 65;
-int g_att3_variant = -1;
-inline int att3_variant() {
-  if (g_att3_variant < 0) {
-    const char* e = getenv("B2E_ATT3");
-    g_att3_variant = e ? atoi(e) : AT3_DEFAULT_VARIANT;
-  }
-  return g_att3_variant;
-}
-
 // Token layout of a forward pass (pack.cuh): null pointers = the padded [B, S] layout.
 struct SeqLayout {
   const int* cu = nullptr;       // [B + 1]
@@ -390,101 +270,82 @@ struct SeqLayout {
   const int* tok_src = nullptr;  // [B * S]
 };
 
-template <int V>
-int launch_attention_v(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnScratch& sc,
-                       const CUtensorMap& tctx, void* ctx, const SeqLayout& lay, int B, int S, int heads,
-                       int grid, float scale_log2e, cudaStream_t st, int window = 0) {
-  if constexpr ((V & 64) != 0) {   // four softmax warpgroups, chunks split by key columns (attention5.cuh)
-    auto kern5 = attention5_d64_kernel<(V & ~64)>;
-    constexpr bool epi = (V & 128) != 0;   // + the epilogue warpgroup
-    constexpr int smem5 = At5Smem<epi>::BYTES;
-    const int arc5 = ensure_smem_attr(kern5, smem5);
-    if (arc5) return arc5;
-    kern5<<<grid, epi ? AT5_THREADS_EPI : AT5_THREADS, smem5, st>>>(tq, tkv, sc.bias, sc.kv_chunks, sc.plain_chunks, tctx, B, S,
-                                                     attn_s_pad(S), heads, scale_log2e, window, lay.cu, lay.len,
-                                                     static_cast<h16*>(ctx));
-    CUDA_TRY(cudaGetLastError());
-    return B2E_OK;
-  }
-  auto kern = attention3_d64_kernel<V>;
-  const int arc = ensure_smem_attr(kern, AT3_SMEM_BYTES);
-  if (arc) return arc;
-  kern<<<grid, AT3_THREADS, AT3_SMEM_BYTES, st>>>(tq, tkv, sc.bias, sc.kv_chunks, sc.plain_chunks, tctx, B, S,
-                                                  attn_s_pad(S), heads, scale_log2e, window, lay.cu, lay.len,
-                                                  static_cast<h16*>(ctx));
+template <int D, int MODE, int V>
+int launch_attention_kernel(const CUtensorMap& tm, const AttnScratch& sc, void* ctx, int B, int S, int heads,
+                            int kv_heads, int window, cudaStream_t st, const SeqLayout& lay) {
+  using Cfg = AtCfg<D, V>;
+  auto kern = attention_kernel<D, MODE, V>;
+  int rc = ensure_smem_attr(kern, Cfg::SMEM_BYTES);
+  if (rc) return rc;
+  CUtensorMap tm_ctx = {};   // [B*S, heads*D], box 64 x 64: the epilogue role's TMA stores
+  if ((V & 128) && (rc = make_tmap_h16(&tm_ctx, ctx, (uint64_t)B * S, (uint64_t)heads * D, 64))) return rc;
+  const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(D));
+  const long long ctas = (long long)heads * B * ((S + Cfg::QT - 1) / Cfg::QT);
+  if (ctas > 0x7fffffffLL)
+    return fail(B2E_ERR_INVALID, "attention: %lld CTAs (heads=%d B=%d S=%d) exceed one grid", ctas, heads, B, S);
+  kern<<<(unsigned)ctas, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(tm, tm_ctx, sc.bias, sc.kv_chunks, sc.plain_chunks, B, S,
+                                                    attn_s_pad(S), heads, kv_heads, window, scale_log2e, lay.cu,
+                                                    lay.len, static_cast<h16*>(ctx));
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
 }
 
-// tq: [T,3H] box 64x128, tkv: [T,3H] box 64x64.  `sc` must have been prepared for this batch's mask.
-// window > 0: bidirectional sliding window |q - k| <= window (ModernBERT's local layers), else full attention.
-int launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnScratch& sc, void* ctx,
-                     int B, int S, int heads, int sms, cudaStream_t st, int window = 0,
-                     const SeqLayout& lay = SeqLayout()) {
-  const float scale_log2e = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-  const int nq = (S + 127) / 128;
-  const long long items = (long long)B * heads * ((nq + 1) / 2);
-  const int grid = items < sms ? (int)items : sms;
-  CUtensorMap tctx;  // [B*S, H]: full 128-row tiles leave through TMA, a sequence's partial last tile row by row
-  int rc;
-  if ((rc = make_tmap_h16(&tctx, ctx, (uint64_t)B * S, (uint64_t)heads * AT3_D, 128))) return rc;
-  if (window > 0) {
-    if ((att3_variant() & 192) == 192)
-      return launch_attention_v<192 + 17>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st, window);
-    if (att3_variant() & 64)
-      return launch_attention_v<64 + 17>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st, window);
-    return launch_attention_v<17>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st, window);
+// Variant of the head_dim-64 kernel (attention.cuh: bit 0 plain chunks from attn_prep, bits 2-3 polynomial
+// exponentials per four, bit 6 four consumer warpgroups, bit 7 epilogue role, bit 8 timeline stamps);
+// B2E_ATT3=<n> or b2e_debug_set_att3_variant picks one of the instantiated ones for A/B measurements.
+// 193 (four warpgroups, plain chunks from attn_prep, TMA-store epilogue role) measured fastest of these at the C2
+// shape (B=512, S=512, 12 heads) on an H100 SXM, all variants side by side in one process: about 6 % ahead of
+// variant 1 (two warpgroups) and 17 % ahead of variant 0; within 3 % of variant 1 at S = 1026.
+constexpr int AT_DEFAULT_VARIANT = 193;
+int g_att3_variant = -1;
+inline int att3_variant() {
+  if (g_att3_variant < 0) {
+    const char* e = getenv("B2E_ATT3");
+    g_att3_variant = e ? atoi(e) : AT_DEFAULT_VARIANT;
   }
-  switch (att3_variant()) {
-    case 0: return launch_attention_v<0>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 1: return launch_attention_v<1>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 2: return launch_attention_v<2>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 3: return launch_attention_v<3>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 7: return launch_attention_v<7>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 11: return launch_attention_v<11>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 5: return launch_attention_v<5>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 33: return launch_attention_v<33>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 37: return launch_attention_v<37>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 41: return launch_attention_v<41>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 45: return launch_attention_v<45>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 64: return launch_attention_v<64>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 65: return launch_attention_v<65>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 69: return launch_attention_v<69>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 73: return launch_attention_v<73>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 193: return launch_attention_v<193>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-    case 261: return launch_attention_v<261>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);   // 5 + timeline stamps
-    case 321: return launch_attention_v<321>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);   // 65 + timeline stamps
-    case 197: return launch_attention_v<197>(tq, tkv, sc, tctx, ctx, lay, B, S, heads, grid, scale_log2e, st);
-  }
-  return fail(B2E_ERR_INVALID, "attention variant %d is not instantiated (0,1,2,3,5,7,11,33,37,41,45,64,65,69,73,193,197,261,321)",
-              att3_variant());
+  return g_att3_variant;
 }
 
-// Causal grouped-query attention, head_dim 128 (attention4.cuh).  qkv is [B*S, (heads + 2 kv_heads)*128]
+// tkv: [T,3H] box 64x64.  `sc` must have been prepared for this batch's mask.
+// window > 0: bidirectional sliding window |q - k| <= window (ModernBERT's local layers), else full attention;
+// the windowed kernel takes the variant's warpgroup count and epilogue role.
+int launch_attention(const CUtensorMap& tkv, const AttnScratch& sc, void* ctx, int B, int S, int heads,
+                     cudaStream_t st, int window = 0, const SeqLayout& lay = SeqLayout()) {
+  const int v = att3_variant();
+#define B2E_ATT(MODE, V) launch_attention_kernel<64, MODE, V>(tkv, sc, ctx, B, S, heads, heads, window, st, lay)
+  if (window > 0) {
+    switch (v & 192) {
+      case 0: return B2E_ATT(1, 0);
+      case 64: return B2E_ATT(1, 64);
+      case 128: return B2E_ATT(1, 128);
+      case 192: return B2E_ATT(1, 192);
+    }
+    return fail(B2E_ERR_INVALID, "windowed attention: variant %d has no instantiation (bits 6-7 of the variant pick "
+                "0, 64, 128 or 192)", v);
+  }
+  switch (v) {
+    case 0: return B2E_ATT(0, 0);
+    case 1: return B2E_ATT(0, 1);
+    case 5: return B2E_ATT(0, 5);
+    case 64: return B2E_ATT(0, 64);
+    case 65: return B2E_ATT(0, 65);
+    case 69: return B2E_ATT(0, 69);
+    case 193: return B2E_ATT(0, 193);
+    case 261: return B2E_ATT(0, 261);   // 5 + timeline stamps
+    case 321: return B2E_ATT(0, 321);   // 65 + timeline stamps
+  }
+#undef B2E_ATT
+  return fail(B2E_ERR_INVALID, "attention variant %d is not instantiated (0,1,5,64,65,69,193,261,321)", v);
+}
+
+// Causal grouped-query attention, head_dim 128.  qkv is [B*S, (heads + 2 kv_heads)*128]
 // with columns  q heads | k heads | v heads;  sc must have been prepared for (mask, B, S).
 int launch_attention_causal_d128(const void* qkv, AttnScratch& sc, void* ctx, int B, int S, int heads,
-                                 int kv_heads, int window, int sms, cudaStream_t st,
-                                 const SeqLayout& lay = SeqLayout()) {
-  {
-    const int arc = ensure_smem_attr(attention4_d128_causal_kernel, AT4_SMEM_BYTES);
-    if (arc) return arc;
-  }
-  const uint64_t ld = (uint64_t)(heads + 2 * kv_heads) * AT4_D;
-  CUtensorMap tq, tkv, tctx;
-  int rc;
-  if ((rc = make_tmap_h16(&tq, qkv, (uint64_t)B * S, ld, 128))) return rc;
-  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, ld, AT4_KC))) return rc;
-  // [B*S, heads*128]: full 128-row tiles leave through TMA, a sequence's partial last tile row by row
-  if ((rc = make_tmap_h16(&tctx, ctx, (uint64_t)B * S, (uint64_t)heads * AT4_D, 128))) return rc;
-  const int nq = (S + 127) / 128;
-  const long long items = (long long)B * heads * ((nq + 1) / 2);
-  const int grid = items < sms ? (int)items : sms;
-  const float scale_log2e = 0.08838834764831845f * 1.4426950408889634f;  // 128^-0.5 * log2(e)
-  attention4_d128_causal_kernel<<<grid, AT4_THREADS, AT4_SMEM_BYTES, st>>>(
-      tq, tkv, sc.bias, sc.kv_chunks, sc.plain_chunks, tctx, B, S, attn_s_pad(S), heads, kv_heads, window,
-      scale_log2e, lay.cu, lay.len, static_cast<h16*>(ctx));
-  CUDA_TRY(cudaGetLastError());
-  return B2E_OK;
+                                 int kv_heads, int window, cudaStream_t st, const SeqLayout& lay = SeqLayout()) {
+  CUtensorMap tm;
+  const int rc = make_tmap_h16(&tm, qkv, (uint64_t)B * S, (uint64_t)(heads + 2 * kv_heads) * 128, AT_KC);
+  if (rc) return rc;
+  return launch_attention_kernel<128, 2, 0>(tm, sc, ctx, B, S, heads, kv_heads, window, st, lay);
 }
 
 #define DISPATCH_NV(H, CALL)                                        \
@@ -815,31 +676,30 @@ int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
   CUDA_TRY(cudaGetLastError());
 
   if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv, tm_kv64;
-  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT3_KC))) return rc;
+  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_kv64;
+  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT_KC))) return rc;
   if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, 128))) return rc;
 
   for (int l = 0; l < d.num_layers; ++l) {
     if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, (const float*)e->L(l, 1), nullptr, M,
-                          3 * H, H, B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+                          3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    if ((rc = launch_attention(tm_qkv, tm_kv64, e->attn, e->ctx, B, S, d.heads, e->sms, st, 0, lay)))
+    if ((rc = launch_attention(tm_kv64, e->attn, e->ctx, B, S, d.heads, st, 0, lay)))
       return rc;
     // the residual add rides on the LayerNorm's coalesced reads, not on the GEMM epilogue
     if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, (const float*)e->L(l, 3), nullptr, M, H, H,
-                          B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+                          B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_NV(H, (layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->tmp, e->hidden, (const float*)e->L(l, 4), (const float*)e->L(l, 5),
                        e->hidden, M, d.eps, lay.t_real)));
     if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, (const float*)e->L(l, 7), nullptr, M, I,
-                          H, B2E_EPI_BIAS_GELU, e->sms, st, lay.t_real)))
+                          H, B2E_EPI_BIAS_GELU, st, lay.t_real)))
       return rc;
     if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, (const float*)e->L(l, 9), nullptr, M, H, I,
-                          B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+                          B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < d.num_layers) {
       DISPATCH_NV(H, (layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
@@ -868,12 +728,11 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
                      lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
   if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv, tm_kv64;
+  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_kv64;
   if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT3_KC))) return rc;
+  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT_KC))) return rc;
 
   DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      e->xres, nullptr, (const float*)e->E(0, 0), (const float*)e->E(0, 1), e->hidden,
@@ -881,23 +740,23 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
   const long long rope_work = (long long)M * d.heads * 2;
   for (int l = 0; l < L; ++l) {
     if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, (const float*)e->E(l, 3), nullptr, M,
-                          3 * H, H, B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+                          3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
         e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
-    if ((rc = launch_attention(tm_qkv, tm_kv64, e->attn, e->ctx, B, S, d.heads, e->sms, st, 0, lay)))
+    if ((rc = launch_attention(tm_kv64, e->attn, e->ctx, B, S, d.heads, st, 0, lay)))
       return rc;
     if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, (const float*)e->E(l, 5), nullptr, M, H, H,
-                          B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+                          B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->E(l, 6), (const float*)e->E(l, 7), e->hidden,
                        M, d.eps, lay.t_real)));
     if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, (const float*)e->E(l, 9), nullptr, M, I, H,
-                          B2E_EPI_BIAS_GELU, e->sms, st, lay.t_real)))
+                          B2E_EPI_BIAS_GELU, st, lay.t_real)))
       return rc;
     if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, (const float*)e->E(l, 11), nullptr, M, H, I,
-                          B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+                          B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
       DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
@@ -933,25 +792,22 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
   const int n_rot = d.heads + d.kv_heads;   // q heads and k heads are adjacent columns of qkv
   const long long rope_work = (long long)M * n_rot;
   for (int l = 0; l < L; ++l) {
-    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, QC, H, B2E_EPI_BIAS,
-                          e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, QC, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     rope_halves_kernel<64><<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
         e->qkv, e->rope_cos, e->rope_sin, M, S, n_rot, QC, lay.t_real, lay.tok_src);
     if ((rc = launch_attention_causal_d128(e->qkv, e->attn, e->ctx, B, S, d.heads, d.kv_heads,
-                                           d.sliding_window, e->sms, st, lay)))
+                                           d.sliding_window, st, lay)))
       return rc;
-    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, CC, B2E_EPI_BIAS,
-                          e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, CC, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_NV(H, (add_rmsnorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->Mi(l, 3), e->hidden, M, d.eps, lay.t_real)));
     // gate and up in one GEMM (interleaved rows), silu(gate) * up in its epilogue: [M, I]
     if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H,
-                          B2E_EPI_SWIGLU, e->sms, st, lay.t_real)))
+                          B2E_EPI_SWIGLU, st, lay.t_real)))
       return rc;
-    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS,
-                          e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
       DISPATCH_NV(H, (add_rmsnorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
@@ -977,12 +833,11 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
                      e->hidden, M, d.eps, lay.t_real, lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
   if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv, tm_kv64;
+  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_kv64;
   if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT3_KC))) return rc;
+  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT_KC))) return rc;
   const long long rope_work = (long long)M * d.heads * 2;
   for (int l = 0; l < L; ++l) {
     const bool global = (l % d.global_every) == 0;
@@ -991,25 +846,23 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
                          e->xres, e->tmp, (const float*)e->Mb(l, 0), (const float*)e->Mb(l, 1), e->hidden, M,
                          d.eps, lay.t_real)));
     }
-    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, 3 * H, H, B2E_EPI_BIAS,
-                          e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, 3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
         e->qkv, global ? e->rope_cos : e->rope_cos2, global ? e->rope_sin : e->rope_sin2, M, S, 2 * d.heads,
         3 * H, lay.t_real, lay.tok_src);
-    if ((rc = launch_attention(tm_qkv, tm_kv64, e->attn, e->ctx, B, S, d.heads, e->sms, st,
+    if ((rc = launch_attention(tm_kv64, e->attn, e->ctx, B, S, d.heads, st,
                                global ? 0 : d.sliding_window, lay)))
       return rc;
-    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, H, B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->Mb(l, 4), (const float*)e->Mb(l, 5), e->hidden, M,
                        d.eps, lay.t_real)));
     // Wi with its input / gate halves interleaved: gelu(input) * gate in the epilogue -> [M, I]
-    if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H, B2E_EPI_GEGLU,
-                          e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H, B2E_EPI_GEGLU, st, lay.t_real)))
       return rc;
-    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, e->sms, st, lay.t_real)))
+    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
   }
   CUDA_TRY(cudaGetLastError());
@@ -1024,18 +877,22 @@ extern "C" {
 int b2e_version(void) { return B2E_ABI_VERSION; }
 int b2e_storage_dtype(void) { return kStorageDtype; }
 
-// Profiling hooks (include/b2e_debug.h, not part of the reference-facing ABI): device buffer of
-// 4 x 256 int64 that CTAs 0 and 1 of the CTA-pair GEMM fill with clock64() stamps ([cta*2 + role][n],
-// role 0 = producer, 1 = MMA).  Same idea for the streaming attention kernel: 3 roles x (256 clocks +
-// 256 event codes) int64.
+// Profiling hooks (include/b2e_debug.h, not part of the reference-facing ABI).
 int b2e_debug_set_att3_clock(void* device_buffer) {
   long long* p = static_cast<long long*>(device_buffer);
-  CUDA_TRY(cudaMemcpyToSymbol(g_att3_clock, &p, sizeof(p)));
+  CUDA_TRY(cudaMemcpyToSymbol(g_att_clock, &p, sizeof(p)));
   return B2E_OK;
 }
 
-int b2e_debug_set_att3_flags(int flags) {
-  CUDA_TRY(cudaMemcpyToSymbol(g_att3_flags, &flags, sizeof(flags)));
+int b2e_debug_set_att3_variant(int variant) {
+  g_att3_variant = variant;
+  return B2E_OK;
+}
+
+int b2e_debug_set_clock_buffer(void* device_buffer) {
+  long long* p = static_cast<long long*>(device_buffer);
+  g_gemm_profiling = p != nullptr;
+  CUDA_TRY(cudaMemcpyToSymbol(g_gemm_clock, &p, sizeof(p)));
   return B2E_OK;
 }
 
@@ -1045,24 +902,6 @@ int b2e_debug_set_packing(int on) {
   return B2E_OK;
 }
 
-int b2e_debug_set_att3_variant(int variant) {
-  g_att3_variant = variant;
-  return B2E_OK;
-}
-
-// Experiment knob for the CTA-pair GEMM: bit 0 = skip the epilogue's math and stores.
-int b2e_debug_set_pair_flags(int flags) {
-  g_gemm2_profiling = flags != 0;
-  CUDA_TRY(cudaMemcpyToSymbol(g_gemm2_flags, &flags, sizeof(flags)));
-  return B2E_OK;
-}
-
-int b2e_debug_set_clock_buffer(void* device_buffer) {
-  long long* p = static_cast<long long*>(device_buffer);
-  g_gemm2_profiling = p != nullptr;
-  CUDA_TRY(cudaMemcpyToSymbol(g_gemm2_clock, &p, sizeof(p)));
-  return B2E_OK;
-}
 // Run only the first n layers from now on (1 <= n <= the model's depth; 0 restores the full depth).  The
 // output is what a checkpoint truncated to n layers would give: BERT's hidden_states[n]; for the pre-norm
 // families the final norm applied to the residual stream after n layers.  Used by tools/drift_report.py.
@@ -1152,10 +991,10 @@ int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_w
   e->sms = info.sms;
   e->tm_wqkv.resize(L); e->tm_wo.resize(L); e->tm_w1.resize(L); e->tm_w2.resize(L);
   for (int l = 0; l < L; ++l) {
-    if ((rc = make_tmap_h16(&e->tm_wqkv[l], e->Mi(l, 1), QC, H, gemm_bn_for(QC))) ||
-        (rc = make_tmap_h16(&e->tm_wo[l], e->Mi(l, 2), H, CC, gemm_bn_for(H))) ||
-        (rc = make_tmap_h16(&e->tm_w1[l], e->Mi(l, 4), 2 * I, H, gemm_bn_for(2 * I))) ||
-        (rc = make_tmap_h16(&e->tm_w2[l], e->Mi(l, 5), H, I, gemm_bn_for(H)))) {
+    if ((rc = make_tmap_h16(&e->tm_wqkv[l], e->Mi(l, 1), QC, H, GEMM_BN)) ||
+        (rc = make_tmap_h16(&e->tm_wo[l], e->Mi(l, 2), H, CC, GEMM_BN)) ||
+        (rc = make_tmap_h16(&e->tm_w1[l], e->Mi(l, 4), 2 * I, H, GEMM_BN)) ||
+        (rc = make_tmap_h16(&e->tm_w2[l], e->Mi(l, 5), H, I, GEMM_BN))) {
       delete e;
       return rc;
     }
@@ -1210,10 +1049,10 @@ int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int
     const void* wo = mbert ? e->Mb(l, 3) : esm ? e->E(l, 4) : e->L(l, 2);
     const void* w1 = mbert ? e->Mb(l, 6) : esm ? e->E(l, 8) : e->L(l, 6);
     const void* w2 = mbert ? e->Mb(l, 7) : esm ? e->E(l, 10) : e->L(l, 8);
-    if ((rc = make_tmap_h16(&e->tm_wqkv[l], wqkv, 3 * H, H, gemm_bn_for(3 * H))) ||
-        (rc = make_tmap_h16(&e->tm_wo[l], wo, H, H, gemm_bn_for(H))) ||
-        (rc = make_tmap_h16(&e->tm_w1[l], w1, n1, H, gemm_bn_for(n1))) ||
-        (rc = make_tmap_h16(&e->tm_w2[l], w2, H, I, gemm_bn_for(H)))) {
+    if ((rc = make_tmap_h16(&e->tm_wqkv[l], wqkv, 3 * H, H, GEMM_BN)) ||
+        (rc = make_tmap_h16(&e->tm_wo[l], wo, H, H, GEMM_BN)) ||
+        (rc = make_tmap_h16(&e->tm_w1[l], w1, n1, H, GEMM_BN)) ||
+        (rc = make_tmap_h16(&e->tm_w2[l], w2, H, I, GEMM_BN))) {
       delete e;
       return rc;
     }
@@ -1640,8 +1479,8 @@ int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* re
   if ((rc = current_device_info(&info))) return rc;
   CUtensorMap ta, tb;
   if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
-  if ((rc = make_tmap_h16(&tb, W, N, K, gemm_bn_for(N)))) return rc;
-  return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, info.sms, (cudaStream_t)stream);
+  if ((rc = make_tmap_h16(&tb, W, N, K, GEMM_BN))) return rc;
+  return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
 }
 
 int b2e_attention_d64(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
@@ -1653,11 +1492,10 @@ int b2e_attention_d64(const void* qkv, const int64_t* mask, void* ctx, int B, in
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  CUtensorMap tq, tkv;
-  if ((rc = make_tmap_h16(&tq, qkv, (uint64_t)B * S, (uint64_t)3 * heads * AT3_D, 128))) return rc;
-  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * AT3_D, AT3_KC))) return rc;
+  CUtensorMap tkv;
+  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * 64, AT_KC))) return rc;
   if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
-  return launch_attention(tq, tkv, g_attn_scratch, ctx, B, S, heads, info.sms, st);
+  return launch_attention(tkv, g_attn_scratch, ctx, B, S, heads, st);
 }
 
 int b2e_attention_d64_window(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
@@ -1668,11 +1506,10 @@ int b2e_attention_d64_window(const void* qkv, const int64_t* mask, void* ctx, in
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  CUtensorMap tq, tkv;
-  if ((rc = make_tmap_h16(&tq, qkv, (uint64_t)B * S, (uint64_t)3 * heads * AT3_D, 128))) return rc;
-  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * AT3_D, AT3_KC))) return rc;
+  CUtensorMap tkv;
+  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * 64, AT_KC))) return rc;
   if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
-  return launch_attention(tq, tkv, g_attn_scratch, ctx, B, S, heads, info.sms, st, window);
+  return launch_attention(tkv, g_attn_scratch, ctx, B, S, heads, st, window);
 }
 
 int b2e_attention_causal_d128(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
@@ -1686,8 +1523,7 @@ int b2e_attention_causal_d128(const void* qkv, const int64_t* mask, void* ctx, i
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
-  return launch_attention_causal_d128(qkv, g_attn_scratch, ctx, B, S, heads, kv_heads, window,
-                                      info.sms, st);
+  return launch_attention_causal_d128(qkv, g_attn_scratch, ctx, B, S, heads, kv_heads, window, st);
 }
 
 // ---- exact inner-product top-k (retrieval query path)

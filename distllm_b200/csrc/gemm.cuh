@@ -1,16 +1,13 @@
-// Persistent warp-specialised h16 GEMM for sm_100a:  out[M,N] = epi(A[M,K] . W[N,K]^T + bias)
+// Warp-specialised h16 GEMM for sm_90a:  out[M,N] = epi(A[M,K] . W[N,K]^T + bias)
 //
-//   warp 0      TMA producer   (one elected lane): A/W tiles -> 128B-swizzled smem ring
-//   warp 1      MMA issuer     (one elected lane): tcgen05.mma 128 x BN x 16, fp32 accum in TMEM
-//   warp 2      TMEM allocator
-//   warps 4-11  epilogue: tcgen05.ld -> +bias (-> erf-GELU | +residual) -> h16 -> per-warp
-//               swizzled smem tile (32 rows x 64 cols) -> TMA store (cp.async.bulk.tensor)
+//   warp 8      TMA producer (one elected lane): 128 x 64 A tile and 128 x 64 W tile per stage into a
+//               128B-swizzled shared-memory ring
+//   warps 0-7   two consumer warpgroups, 64 output rows each: wgmma m64n128k16 with both operands read
+//               from shared memory, fp32 accumulators in registers; the epilogue (+bias, erf-GELU |
+//               +residual | gated activation) runs on those registers and stores h16 pairs
 //
-// The accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps
-// the MMAs of tile i+1.  Output goes through TMA stores because direct "one row per lane" global
-// stores cost 32 L1 wavefronts per instruction and, at 4096 wavefronts per 128x256 tile, fought the
-// tensor core's own shared-memory operand reads for the L1/smem data pipe (ncu: lsu wavefronts
-// 40-55 % + tc wavefronts 20-52 % of the pipe, profiles/r01_ncu_v1_summary.md).
+// One CTA per 128 x 128 output tile; three 32 KiB stages keep two CTAs resident per SM, so the epilogue
+// of one overlaps the main loop of the other.
 //
 // This replaces the cuBLAS nn.Linear calls HF BERT issues from
 // transformers/models/bert/modeling_bert.py:180-182 (q,k,v), :294-298 (attn out), :339-342 (FFN up +
@@ -30,24 +27,15 @@ enum GemmEpi : int { EPI_BIAS = 0, EPI_BIAS_GELU = 1, EPI_BIAS_RESID = 2, EPI_SW
 __host__ __device__ constexpr bool epi_is_glu(int epi) { return epi == EPI_SWIGLU || epi == EPI_GEGLU; }
 
 constexpr int GEMM_BM = 128;
+constexpr int GEMM_BN = 128;
 constexpr int GEMM_BK = 64;  // 64 h16 = one 128-byte swizzle row
-constexpr int GEMM_THREADS = 384;
-constexpr int GEMM_EPI_WARPS = 8;
-constexpr int GEMM_OUT_BOX_ROWS = 32;   // TMA store box: 64 columns x 32 rows (one warp's chunk)
-constexpr int GEMM_STAGING_BYTES = GEMM_OUT_BOX_ROWS * 128;  // 4 KiB per epilogue warp
-
-template <int BN, int STAGES>
-struct GemmCfg {
-  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-  static constexpr int B_BYTES = BN * GEMM_BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGING_OFFSET = STAGES * STAGE_BYTES;  // 1024-aligned (stage sizes are)
-  static constexpr int BAR_OFFSET = STAGING_OFFSET + GEMM_EPI_WARPS * GEMM_STAGING_BYTES;
-  static constexpr int BIAS_OFFSET = BAR_OFFSET + 256;         // [2][BN] fp32 bias slices
-  static constexpr int SMEM_BYTES = BIAS_OFFSET + 2 * BN * 4;  // dynamic smem must start 1024-aligned
-  static constexpr int TMEM_COLS = 2 * BN;
-  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KiB per-CTA shared memory limit");
-};
+constexpr int GEMM_STAGES = 3;
+constexpr int GEMM_THREADS = 288;   // two consumer warpgroups + the producer warp
+constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;
+constexpr int GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_BN * GEMM_BK * 2;
+constexpr int GEMM_BAR_OFFSET = GEMM_STAGES * GEMM_STAGE_BYTES;
+constexpr int GEMM_SMEM_BYTES = GEMM_BAR_OFFSET + 64 + 1024;   // + slack to align the ring to 1024 B
+static_assert(2 * GEMM_SMEM_BYTES <= 232448, "two CTAs per SM");
 
 // erf-GELU, x * Phi(x), with Phi from the Abramowitz-Stegun 7.1.26 erfc polynomial
 // (|erf error| <= 1.5e-7): gelu(x) = max(x,0) - 0.5*|x|*poly(t)*exp(-x^2/2), t = 1/(1 + p*|x|/sqrt2).
@@ -82,314 +70,143 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaxf(x, 0.0f) - 0.5f * ax * p * e;
 }
 
-// Epilogue of one 32-row x 64-column chunk held as two 32-column TMEM reads: bias (+GELU / +resid),
-// h16, into the warp's swizzled staging tile (row = lane).  `resid_row` points at this lane's
-// row, first column of the chunk (only read when EPI == EPI_BIAS_RESID and the row exists).
-template <int EPI>
-__device__ __forceinline__ void gemm_epilogue_chunk(const uint32_t (&acc)[2][32],
-                                                    const float* __restrict__ bias_smem,
-                                                    const h16* __restrict__ resid_row, bool row_ok,
-                                                    uint8_t* staging, int lane) {
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {  // 16-byte unit = 8 columns
-    const float4 b0 = *reinterpret_cast<const float4*>(bias_smem + u * 8);
-    const float4 b1 = *reinterpret_cast<const float4*>(bias_smem + u * 8 + 4);
-    const uint32_t* a = &acc[u >> 2][(u & 3) * 8];
-    float v[8];
-    v[0] = __uint_as_float(a[0]) + b0.x;
-    v[1] = __uint_as_float(a[1]) + b0.y;
-    v[2] = __uint_as_float(a[2]) + b0.z;
-    v[3] = __uint_as_float(a[3]) + b0.w;
-    v[4] = __uint_as_float(a[4]) + b1.x;
-    v[5] = __uint_as_float(a[5]) + b1.y;
-    v[6] = __uint_as_float(a[6]) + b1.z;
-    v[7] = __uint_as_float(a[7]) + b1.w;
-    if (EPI == EPI_BIAS_GELU) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-#ifdef B2E_GELU_TWO_MUFU
-        v[e] = gelu_erf(v[e]);
-#else
-        v[e] = gelu_erf_fast(v[e]);
-#endif
-      }
-    }
-    if (EPI == EPI_BIAS_RESID) {
-      if (row_ok) {
-        const uint4 rr = *reinterpret_cast<const uint4*>(resid_row + u * 8);
-        const float2 r0 = unpack_h16x2(rr.x), r1 = unpack_h16x2(rr.y), r2 = unpack_h16x2(rr.z),
-                     r3 = unpack_h16x2(rr.w);
-        v[0] += r0.x; v[1] += r0.y; v[2] += r1.x; v[3] += r1.y;
-        v[4] += r2.x; v[5] += r2.y; v[6] += r3.x; v[7] += r3.y;
-      }
-    }
-    uint4 o;
-    o.x = pack_h16x2(v[0], v[1]);
-    o.y = pack_h16x2(v[2], v[3]);
-    o.z = pack_h16x2(v[4], v[5]);
-    o.w = pack_h16x2(v[6], v[7]);
-    // 128B-swizzle: unit index XOR (row & 7) -- conflict-free for "one row per lane" writes and
-    // exactly the layout the SWIZZLE_128B tensor map expects
-    *reinterpret_cast<uint4*>(staging + lane * 128 + ((u ^ (lane & 7)) << 4)) = o;
-  }
+__device__ __forceinline__ float silu(float x) {
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + fast_exp2(-1.4426950408889634f * x)));
+  return x * r;
 }
 
-// Same chunk epilogue with the bias slice read straight from global memory (all lanes read the same
-// 16 float4: L1 broadcast hits), no shared-memory bias tile and no barrier among the epilogue warps.
-template <int EPI>
-__device__ __forceinline__ void gemm_epilogue_chunk_gbias(const uint32_t (&acc)[2][32],
-                                                          const float* __restrict__ bias,
-                                                          const h16* __restrict__ resid_row,
-                                                          bool row_ok, uint8_t* staging, int lane) {
-#pragma unroll
-  for (int u = 0; u < 8; ++u) {
-    float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
-    if (bias != nullptr) {
-      b0 = __ldg(reinterpret_cast<const float4*>(bias + u * 8));
-      b1 = __ldg(reinterpret_cast<const float4*>(bias + u * 8 + 4));
-    }
-    const uint32_t* a = &acc[u >> 2][(u & 3) * 8];
-    float v[8];
-    v[0] = __uint_as_float(a[0]) + b0.x;
-    v[1] = __uint_as_float(a[1]) + b0.y;
-    v[2] = __uint_as_float(a[2]) + b0.z;
-    v[3] = __uint_as_float(a[3]) + b0.w;
-    v[4] = __uint_as_float(a[4]) + b1.x;
-    v[5] = __uint_as_float(a[5]) + b1.y;
-    v[6] = __uint_as_float(a[6]) + b1.z;
-    v[7] = __uint_as_float(a[7]) + b1.w;
-    if (EPI == EPI_BIAS_GELU) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] = gelu_erf_fast(v[e]);
-    }
-    if (EPI == EPI_BIAS_RESID) {
-      if (row_ok) {
-        const uint4 rr = *reinterpret_cast<const uint4*>(resid_row + u * 8);
-        const float2 r0 = unpack_h16x2(rr.x), r1 = unpack_h16x2(rr.y), r2 = unpack_h16x2(rr.z),
-                     r3 = unpack_h16x2(rr.w);
-        v[0] += r0.x; v[1] += r0.y; v[2] += r1.x; v[3] += r1.y;
-        v[4] += r2.x; v[5] += r2.y; v[6] += r3.x; v[7] += r3.y;
-      }
-    }
-    uint4 o;
-    o.x = pack_h16x2(v[0], v[1]);
-    o.y = pack_h16x2(v[2], v[3]);
-    o.z = pack_h16x2(v[4], v[5]);
-    o.w = pack_h16x2(v[6], v[7]);
-    *reinterpret_cast<uint4*>(staging + lane * 128 + ((u ^ (lane & 7)) << 4)) = o;
-  }
-}
+// profiling aid (b2e_debug_set_clock_buffer): CTA 0 of the TL instantiation records clock64() once per
+// K block in the producer ([0][n], after issuing the loads) and in the first consumer warpgroup ([1][n], when
+// the block's MMAs have been retired); 4 x 256 int64
+__device__ long long* g_gemm_clock = nullptr;
 
-// SwiGLU epilogue of one 32-row x 64-output chunk: g, u = the gate / up accumulators (two 32-column
-// TMEM reads each); silu(g) * u -> h16 -> the warp's swizzled staging tile.
-// silu(g) = g / (1 + 2^(-g log2 e)): one ex2 + one rcp per element (hidden under the K loop's MMAs).
-template <bool GELU>
-__device__ __forceinline__ void gemm_swiglu_chunk(const uint32_t (&g)[2][32],
-                                                  const uint32_t (&u)[2][32], uint8_t* staging,
-                                                  int lane) {
-#pragma unroll
-  for (int un = 0; un < 8; ++un) {
-    const uint32_t* gg = &g[un >> 2][(un & 3) * 8];
-    const uint32_t* uu = &u[un >> 2][(un & 3) * 8];
-    float v[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float x = __uint_as_float(gg[e]);
-      if (GELU) {
-        v[e] = gelu_erf_fast(x) * __uint_as_float(uu[e]);
-      } else {
-        float r;
-        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + fast_exp2(-1.4426950408889634f * x)));
-        v[e] = x * r * __uint_as_float(uu[e]);
-      }
-    }
-    uint4 o;
-    o.x = pack_h16x2(v[0], v[1]);
-    o.y = pack_h16x2(v[2], v[3]);
-    o.z = pack_h16x2(v[4], v[5]);
-    o.w = pack_h16x2(v[6], v[7]);
-    *reinterpret_cast<uint4*>(staging + lane * 128 + ((un ^ (lane & 7)) << 4)) = o;
-  }
-}
-
-template <int BN, int STAGES, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_h16_tcgen05_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
-                         const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x BN
-                         const __grid_constant__ CUtensorMap tm_out,  // [M,N] box 64 x 32
-                         const float* __restrict__ bias, const h16* __restrict__ resid, int M,
-                         int N, int K, const int* __restrict__ m_dev) {
+template <int EPI, bool TL = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 2)
+gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
+                      const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x 128
+                      h16* __restrict__ out, const float* __restrict__ bias, const h16* __restrict__ resid,
+                      int M, int N, int K, const int* __restrict__ m_dev) {
   if (m_dev != nullptr) M = __ldg(m_dev);   // device-resident row count (packed token layout)
-  using Cfg = GemmCfg<BN, STAGES>;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t smem_base = smem_u32(smem);
-  if ((smem_base & 1023u) != 0) __trap();  // the swizzled tiles need a 1024-byte aligned base
-
-  const uint32_t full_bar = smem_base + Cfg::BAR_OFFSET;
-  const uint32_t empty_bar = full_bar + 8u * STAGES;
-  const uint32_t tfull_bar = empty_bar + 8u * STAGES;
-  const uint32_t tempty_bar = tfull_bar + 16u;
-  volatile uint32_t* tmem_slot =
-      reinterpret_cast<volatile uint32_t*>(smem + Cfg::BAR_OFFSET + 8 * (2 * STAGES + 4));
-
+  // one-dimensional grid, N tiles fastest: the CTAs resident together share their A rows in L2
+  const int n_blk = static_cast<int>(blockIdx.x % (N / GEMM_BN)), m_blk = static_cast<int>(blockIdx.x / (N / GEMM_BN));
+  if (m_blk * GEMM_BM >= M) return;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t sb = (raw + 1023u) & ~1023u;   // the swizzled tiles need a 1024-byte aligned base
+  const uint32_t full_bar = sb + GEMM_BAR_OFFSET;
+  const uint32_t empty_bar = full_bar + 8u * GEMM_STAGES;
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int kblocks = K / GEMM_BK;
 
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tm_a);
-    tma_prefetch_desc(&tm_b);
-    tma_prefetch_desc(&tm_out);
-  }
-  if (warp == 1 && elect_one()) {
-    for (int s = 0; s < STAGES; ++s) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < GEMM_STAGES; ++s) {
       mbar_init(full_bar + 8u * s, 1);
-      mbar_init(empty_bar + 8u * s, 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar + 8u * s, 1);
-      mbar_init(tempty_bar + 8u * s, GEMM_EPI_WARPS);
+      mbar_init(empty_bar + 8u * s, 2);   // one arrival per consumer warpgroup
     }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  const int m_tiles = (M + GEMM_BM - 1) / GEMM_BM;
-  const int n_tiles = N / BN;
-  const int total_tiles = m_tiles * n_tiles;
-  const int kblocks = K / GEMM_BK;
-
-  if (warp == 0) {
+  long long* clk = (TL && blockIdx.x == 0) ? g_gemm_clock : nullptr;
+  if (warp == 8) {
     if (elect_one()) {
+      tma_prefetch_desc(&tm_a);
+      tma_prefetch_desc(&tm_b);
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-        // (An L2 prefetch of the next tile's A rows -- cp.async.bulk.prefetch.tensor, burst or paced
-        // one per K block -- was measured 8-12 % SLOWER than no prefetch: profiles/r01_gemm_notes.md.)
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
-          const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t fb = full_bar + 8u * stage;
-          mbar_expect_tx(fb, Cfg::STAGE_BYTES);
-          tma_load_2d(a_dst, &tm_a, fb, kb * GEMM_BK, m_blk * GEMM_BM);
-          tma_load_2d(a_dst + Cfg::A_BYTES, &tm_b, fb, kb * GEMM_BK, n_blk * BN);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
+        const uint32_t dst = sb + stage * GEMM_STAGE_BYTES;
+        const uint32_t fb = full_bar + 8u * stage;
+        mbar_expect_tx(fb, GEMM_STAGE_BYTES);
+        tma_load_2d(dst, &tm_a, fb, kb * GEMM_BK, m_blk * GEMM_BM);
+        tma_load_2d(dst + GEMM_A_BYTES, &tm_b, fb, kb * GEMM_BK, n_blk * GEMM_BN);
+        if (TL && clk != nullptr && kb < 256) clk[kb] = clock64();
+        if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_h16(GEMM_BM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++local) {
-        const int as = local & 1;
-        const uint32_t aphase = (local >> 1) & 1u;
-        mbar_wait(tempty_bar + 8u * as, aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * BN);
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(full_bar + 8u * stage, phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t a_desc = make_smem_desc_sw128(a_addr, 16, 1024);
-          const uint64_t b_desc = make_smem_desc_sw128(a_addr + Cfg::A_BYTES, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            // +32 bytes along K inside the swizzle atom == +2 in the (addr >> 4) field
-            tc_mma_f16_ss(d_tmem, a_desc + 2u * k, b_desc + 2u * k, idesc,
-                          static_cast<uint32_t>((kb | k) != 0));
-          }
-          tc_commit(empty_bar + 8u * stage);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        tc_commit(tfull_bar + 8u * as);
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;               // TMEM lane quarter this warp may touch
-    const int half = (warp - 4) >> 2;     // which half of the BN columns
-    constexpr int COLS_PER_WARP = BN / 2;
-    constexpr int NCHUNK = COLS_PER_WARP / 64;  // 64-column chunks (one swizzle atom wide)
-    const int etid = threadIdx.x - 128;   // 0..255 among the epilogue threads
-    float* sbias = reinterpret_cast<float*>(smem + Cfg::BIAS_OFFSET);  // [2][BN]
-    uint8_t* staging = smem + Cfg::STAGING_OFFSET + (warp - 4) * GEMM_STAGING_BYTES;
-    const uint32_t staging_addr = smem_base + Cfg::STAGING_OFFSET + (warp - 4) * GEMM_STAGING_BYTES;
-    int local = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++local) {
-      const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-      const int as = local & 1;
-      const uint32_t aphase = (local >> 1) & 1u;
-      const int row0 = m_blk * GEMM_BM + q * 32;   // first row of this warp's 32-row band
-      const int row = row0 + lane;
-      const bool row_ok = row < M;
-      const int col0 = half * COLS_PER_WARP;       // first column of this warp inside the tile
-      const int gcol0 = n_blk * BN + col0;
-      const h16* resid_row =
-          (EPI == EPI_BIAS_RESID) ? resid + static_cast<size_t>(row) * N + gcol0 : nullptr;
-
-      // the tile's bias slice goes to smem before the accumulator wait (double-buffered by `as`)
-      if (!epi_is_glu(EPI)) {
-        for (int i = etid; i < BN; i += GEMM_EPI_WARPS * 32)
-          sbias[as * BN + i] = (bias != nullptr) ? __ldg(bias + n_blk * BN + i) : 0.0f;
-        asm volatile("bar.sync 1, %0;" ::"n"(GEMM_EPI_WARPS * 32) : "memory");
-      }
-
-      mbar_wait(tfull_bar + 8u * as, aphase);
-      tc_fence_after();
-      const uint32_t t_base = tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                              static_cast<uint32_t>(as * BN + col0);
-      if constexpr (epi_is_glu(EPI)) {
-        static_assert(!epi_is_glu(EPI) || BN == 256, "SwiGLU epilogue: 128 columns per warp");
-        uint32_t g[2][32], u[2][32];
-        tmem_ld32(t_base, g[0]);
-        tmem_ld32(t_base + 32u, g[1]);
-        tmem_ld32(t_base + 64u, u[0]);
-        tmem_ld32(t_base + 96u, u[1]);
-        if (lane == 0) tma_store_wait_read<0>();
-        __syncwarp();
-        tmem_ld_wait();
-        gemm_swiglu_chunk<EPI == EPI_GEGLU>(g, u, staging, lane);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tm_out, staging_addr, n_blk * (BN / 2) + half * 64, row0);
-          tma_store_commit();
-        }
-      }
-#pragma unroll 1
-      for (int c = 0; c < (epi_is_glu(EPI) ? 0 : NCHUNK); ++c) {
-        uint32_t acc[2][32];
-        tmem_ld32(t_base + static_cast<uint32_t>(c * 64), acc[0]);
-        tmem_ld32(t_base + static_cast<uint32_t>(c * 64 + 32), acc[1]);
-        // the previous TMA store must have finished READING the staging tile before we overwrite it
-        if (lane == 0) tma_store_wait_read<0>();
-        __syncwarp();
-        tmem_ld_wait();
-        gemm_epilogue_chunk<EPI>(acc, sbias + as * BN + col0 + c * 64, resid_row + c * 64, row_ok,
-                                 staging, lane);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tm_out, staging_addr, gcol0 + c * 64, row0);  // rows >= M are clipped
-          tma_store_commit();
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar + 8u * as);
-    }
-    if (lane == 0) tma_store_wait_all();  // stores complete before the CTA's smem goes away
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  const int wg = warp >> 2;                  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
+  const int t = threadIdx.x & 127;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  int stage = 0;
+  uint32_t phase = 0;
+  int prev = -1;
+  for (int kb = 0; kb < kblocks; ++kb) {
+    mbar_wait(full_bar + 8u * stage, phase);
+    const uint32_t a_addr = sb + stage * GEMM_STAGE_BYTES + wg * (64 * 128);
+    const uint64_t a_desc = make_smem_desc_sw128(a_addr);
+    const uint64_t b_desc = make_smem_desc_sw128(sb + stage * GEMM_STAGE_BYTES + GEMM_A_BYTES);
+    reg_fence(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_64x128_ss(acc, a_desc + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+    wgmma_commit();
+    reg_fence(acc);
+    // keep one stage of MMAs in flight: the previous one has finished reading its operands
+    wgmma_wait<1>();
+    reg_fence(acc);
+    if (prev >= 0 && t == 0) mbar_arrive(empty_bar + 8u * prev);
+    if (TL && clk != nullptr && threadIdx.x == 0 && kb < 256) clk[256 + kb] = clock64();
+    prev = stage;
+    if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  reg_fence(acc);
+
+  const int r_lo = m_blk * GEMM_BM + wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int c_in = 2 * (t & 3);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int row = r_lo + 8 * half;
+    if (row >= M) continue;
+    if constexpr (epi_is_glu(EPI)) {
+      const int n_out = N / 2;
+      h16* orow = out + static_cast<size_t>(row) * n_out + n_blk * (GEMM_BN / 2);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float g0 = acc[4 * j + 2 * half], g1 = acc[4 * j + 2 * half + 1];
+        const float u0 = acc[4 * (j + 8) + 2 * half], u1 = acc[4 * (j + 8) + 2 * half + 1];
+        float v0, v1;
+        if (EPI == EPI_GEGLU) {
+          v0 = gelu_erf_fast(g0) * u0;
+          v1 = gelu_erf_fast(g1) * u1;
+        } else {
+          v0 = silu(g0) * u0;
+          v1 = silu(g1) * u1;
+        }
+        *reinterpret_cast<uint32_t*>(orow + 8 * j + c_in) = pack_h16x2(v0, v1);
+      }
+    } else {
+      const int col0 = n_blk * GEMM_BN + c_in;
+      h16* orow = out + static_cast<size_t>(row) * N + col0;
+      const h16* rrow = (EPI == EPI_BIAS_RESID) ? resid + static_cast<size_t>(row) * N + col0 : nullptr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+        if (bias != nullptr) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * j));
+          v0 += b.x;
+          v1 += b.y;
+        }
+        if (EPI == EPI_BIAS_GELU) {
+          v0 = gelu_erf_fast(v0);
+          v1 = gelu_erf_fast(v1);
+        }
+        if (EPI == EPI_BIAS_RESID) {
+          const float2 r = unpack_h16x2(*reinterpret_cast<const uint32_t*>(rrow + 8 * j));
+          v0 += r.x;
+          v1 += r.y;
+        }
+        *reinterpret_cast<uint32_t*>(orow + 8 * j) = pack_h16x2(v0, v1);
+      }
+    }
+  }
 }
 
 }  // namespace b2e

@@ -581,8 +581,7 @@ __global__ void rope_table_kernel(float* __restrict__ cos_t, float* __restrict__
 // start at column 0: Q heads directly followed by the K heads in every layout this library uses.
 // A thread owns 8 consecutive frequencies (one 16-byte vector from each half), HALF / 8 threads share a head,
 // so a warp moves 1 KiB (HALF = 32) or 2 x 512 B (HALF = 64) of contiguous bytes per access: the kernel is a plain
-// HBM stream (the first version, one 2-byte element per lane, ran at a quarter of the roofline and cost 13 % of
-// the ESM2-650M step, profiles/r02_ncu_launches_c5.md).
+// HBM stream (one 2-byte element per lane would leave most of each 32-byte sector transfer unused).
 template <int HALF>
 __global__ void __launch_bounds__(256)
 rope_halves_kernel(h16* __restrict__ qkv, const float* __restrict__ cos_t, const float* __restrict__ sin_t,

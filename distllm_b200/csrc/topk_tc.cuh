@@ -5,8 +5,8 @@
 //
 //   1. tf32_scan_kernel      S[n, q] ~ <corpus_n, query_q> for all rows and up to 16 queries per pass: persistent
 //                            CTAs, TMA streams 128-row x 32-float corpus tiles (and the matching 16 x 32 query
-//                            slice) through an 8-stage ring, one thread issues tcgen05.mma.kind::tf32 128x16x8,
-//                            four epilogue warps move the 128 x 16 accumulator to the score matrix.  HBM-bound:
+//                            slice) through an 8-stage ring, one warpgroup runs wgmma m64n16k8 (tf32) on both
+//                            64-row halves of a tile and writes the 128 x 16 accumulator to the score matrix.  HBM-bound:
 //                            N * H * 4 bytes in, N * 64 bytes out.
 //   2. score_hist_kernel     per query a 2048-bin LINEAR histogram of S over [-R, R], R = |q| * max_n |corpus_n|
 //                            (Cauchy-Schwarz: no score lies outside).
@@ -34,79 +34,38 @@ constexpr int TC_A_BYTES = TC_ROWS * TC_KB * 4;    // 16 KiB
 constexpr int TC_B_BYTES = TC_NQ * TC_KB * 4;      // 2 KiB
 constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;
 constexpr int TC_SMEM_BAR = TC_STAGES * TC_STAGE_BYTES;
-constexpr int TC_SMEM_BYTES = TC_SMEM_BAR + 256;
-constexpr int TC_THREADS = 192;              // warp 0 loader, warp 1 MMA issuer, warps 2-5 epilogue
+constexpr int TC_THREADS = 160;              // warps 0-3: the MMA warpgroup, warp 4: TMA loader
 constexpr int TC_BINS = 2048;
 constexpr int TC_MAX_CAND = 4096;
+constexpr int TC_SMEM_BYTES = TC_SMEM_BAR + 256 + 1024;   // + slack to align the ring to 1024 B
 static_assert(TC_STAGE_BYTES % 1024 == 0, "swizzled tiles need 1024-byte alignment");
-
-// kind::tf32 instruction descriptor: D f32, A / B tf32 (format 2), both K-major
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-__device__ __forceinline__ void tc_mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
 
 // scores [tiles * 128, 16]: row n, query q at n * 16 + q (rows >= N come out 0: the TMA zero-fills them)
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tf32_scan_kernel(const __grid_constant__ CUtensorMap tm_corpus,    // [N, H] f32, box 32 x 128
                  const __grid_constant__ CUtensorMap tm_queries,   // [16, H] f32 (zero rows beyond nq), box 32 x 16
                  float* __restrict__ scores, long long tiles, int H) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t sb = smem_u32(smem);
-  if ((sb & 1023u) != 0) __trap();
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5;
   const uint32_t full = sb + TC_SMEM_BAR;              // [STAGES]
   const uint32_t empty = full + 8 * TC_STAGES;         // [STAGES]
-  const uint32_t acc_full = empty + 8 * TC_STAGES;     // [2]
-  const uint32_t acc_empty = acc_full + 16;            // [2]
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + TC_SMEM_BAR + 192);
   const int kblocks = H / TC_KB;
 
-  if (warp == 0) {
-    if (elect_one()) {
-      tma_prefetch_desc(&tm_corpus);
-      tma_prefetch_desc(&tm_queries);
-      for (int i = 0; i < TC_STAGES; ++i) {
-        mbar_init(full + 8u * i, 1);
-        mbar_init(empty + 8u * i, 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(acc_full + 8u * i, 1);
-        mbar_init(acc_empty + 8u * i, 128);
-      }
-      mbar_fence_init();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < TC_STAGES; ++i) {
+      mbar_init(full + 8u * i, 1);
+      mbar_init(empty + 8u * i, 1);
     }
-    __syncwarp();
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), 32);
+    mbar_fence_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       // ---------------------------------------------------------------- loader
+      tma_prefetch_desc(&tm_corpus);
+      tma_prefetch_desc(&tm_queries);
       uint32_t c = 0;
       for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         for (int kb = 0; kb < kblocks; ++kb, ++c) {
@@ -121,56 +80,48 @@ tf32_scan_kernel(const __grid_constant__ CUtensorMap tm_corpus,    // [N, H] f32
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // ---------------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc = make_idesc_tf32(TC_ROWS, TC_NQ);
-      uint32_t c = 0;
-      uint32_t t = 0;
-      for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++t) {
-        const uint32_t buf = t & 1u;
-        if (t >= 2) mbar_wait(acc_empty + 8u * buf, ((t >> 1) - 1) & 1u);
-        tc_fence_after();
-        const uint32_t d = tmem_base + buf * TC_NQ;
-        for (int kb = 0; kb < kblocks; ++kb, ++c) {
-          const int st = c % TC_STAGES;
-          mbar_wait(full + 8u * st, (c / TC_STAGES) & 1u);
-          tc_fence_after();
-          const uint32_t a_addr = sb + st * TC_STAGE_BYTES;
-          const uint64_t a_desc = make_smem_desc_sw128(a_addr, 16, 1024);
-          const uint64_t b_desc = make_smem_desc_sw128(a_addr + TC_A_BYTES, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < TC_KB / 8; ++k)   // 8 floats = 32 bytes per MMA: +2 in the descriptor's 16-byte units
-            tc_mma_tf32_ss(d, a_desc + 2u * k, b_desc + 2u * k, idesc, static_cast<uint32_t>((kb | k) != 0));
-          tc_commit(empty + 8u * st);
-        }
-        tc_commit(acc_full + 8u * buf);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue: TMEM -> score matrix
-    const int quarter = warp & 3;   // TMEM lanes this warp may read
-    const int lane = threadIdx.x & 31;
-    uint32_t t = 0;
-    for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++t) {
-      const uint32_t buf = t & 1u;
-      mbar_wait(acc_full + 8u * buf, (t >> 1) & 1u);
-      tc_fence_after();
-      uint32_t v[16];
-      tmem_ld16(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + buf * TC_NQ, v);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(acc_empty + 8u * buf);
-      float4* dst = reinterpret_cast<float4*>(scores + (static_cast<size_t>(tile) * TC_ROWS + quarter * 32 + lane) * TC_NQ);
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        dst[i] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                             __uint_as_float(v[4 * i + 3]));
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 32);
+  // ------------------------------------------------------------------ MMA warpgroup + epilogue
+  const int t = threadIdx.x;
+  uint32_t c = 0;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    float acc[2][8];
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[hf][i] = 0.0f;
+    for (int kb = 0; kb < kblocks; ++kb, ++c) {
+      const int st = c % TC_STAGES;
+      mbar_wait(full + 8u * st, (c / TC_STAGES) & 1u);
+      const uint32_t a_addr = sb + st * TC_STAGE_BYTES;
+      const uint64_t b_desc = make_smem_desc_sw128(a_addr + TC_A_BYTES);
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_KB / 8; ++k)   // 8 floats = 32 bytes per MMA: +2 in the descriptor's 16-byte units
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf)
+          wgmma_64x16_tf32(acc[hf], make_smem_desc_sw128(a_addr + hf * (64 * 128)) + 2u * k, b_desc + 2u * k,
+                           (kb | k) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      if (t == 0) mbar_arrive(empty + 8u * st);
+    }
+    // accumulator layout (common.cuh): rows 16 (t / 32) + (t % 32) / 4 (+ 8), query columns 8 j + 2 (t % 4)
+    const size_t r_lo = static_cast<size_t>(tile) * TC_ROWS + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int r8 = 0; r8 < 2; ++r8)
+          *reinterpret_cast<float2*>(scores + (r_lo + 64 * hf + 8 * r8) * TC_NQ + 8 * j + 2 * (t & 3)) =
+              make_float2(acc[hf][4 * j + 2 * r8], acc[hf][4 * j + 2 * r8 + 1]);
+  }
 }
 
 // max over rows of |row|^2 (fp32): what bounds every score by Cauchy-Schwarz.  One warp per row, atomicMax on the

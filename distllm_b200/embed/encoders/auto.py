@@ -1,4 +1,4 @@
-"""``auto`` encoder: HuggingFace checkpoint in, native sm_100a forward pass out.
+"""``auto`` encoder: HuggingFace checkpoint in, native sm_90a forward pass out.
 
 Drop-in for distllm/embed/encoders/auto.py:15-138 -- same config fields and defaults, same
 properties, ``encode`` returns the last hidden state ``[B,S,H]``.  transformers is used only to read
@@ -59,7 +59,7 @@ class AutoEncoder:
         hf_config = AutoConfig.from_pretrained(config.pretrained_model_name_or_path)
         if hf_config.model_type not in _SUPPORTED_MODEL_TYPES:
             raise NotImplementedError(
-                f'model_type={hf_config.model_type!r} has no native sm_100a forward pass yet '
+                f'model_type={hf_config.model_type!r} has no native sm_90a forward pass yet '
                 f'(built: {_SUPPORTED_MODEL_TYPES}); there is no eager fallback.',
             )
         _NATIVE_BY_MODEL_TYPE[hf_config.model_type].validate(hf_config)   # before any weight is loaded

@@ -1,4 +1,4 @@
-"""``esm2`` encoder: HuggingFace ESM-2 checkpoint in, native sm_100a forward pass out.
+"""``esm2`` encoder: HuggingFace ESM-2 checkpoint in, native sm_90a forward pass out.
 
 Drop-in for distllm/embed/encoders/esm2.py:15-134 (same config fields and defaults; ``faesm`` is
 accepted and ignored -- the native path replaces both the eager and the flash-attention variants).

@@ -12,7 +12,7 @@ from distllm_b200.embed.encoders import weights as W
 
 
 class NativeBertEncoder:
-    """Encoder forward pass on libb2e (tcgen05 GEMMs + fused attention + row kernels).
+    """Encoder forward pass on libb2e (wgmma GEMMs + fused attention + row kernels).
 
     Holds the device weight tensors (the C handle only borrows their pointers) and wraps
     ``b2e_encode`` / ``b2e_encode_pooled`` / ``b2e_embed_host``.  ``_DESC`` / ``_WEIGHTS`` pick the
@@ -29,7 +29,7 @@ class NativeBertEncoder:
         lib = _native.load(self.storage)
         if not torch.cuda.is_available():
             raise _native.NativeError(
-                'no CUDA device: the native encoder has no CPU fallback (sm_100a only)')
+                'no CUDA device: the native encoder has no CPU fallback (sm_90a only)')
         self.device = torch.device(device if device is not None else f'cuda:{torch.cuda.current_device()}')
         if self.device.index is None:
             self.device = torch.device('cuda', torch.cuda.current_device())
@@ -155,7 +155,7 @@ class NativeEsm2Encoder(NativeBertEncoder):
 
 class NativeMistralEncoder(NativeBertEncoder):
     """Mistral family (pre-RMSNorm blocks, rotary, grouped-query causal attention with optional sliding
-    window, SwiGLU) on the tcgen05 GEMM + the head_dim-128 causal attention kernel; ``token_type_ids``
+    window, SwiGLU) on the wgmma GEMM + the head_dim-128 causal attention kernel; ``token_type_ids``
     unused."""
 
     _DESC = staticmethod(W.mistral_desc)
@@ -165,7 +165,7 @@ class NativeMistralEncoder(NativeBertEncoder):
 
 class NativeModernBertEncoder(NativeBertEncoder):
     """ModernBERT (pre-LayerNorm blocks, rotary with one base per layer type, alternating full / sliding-window
-    bidirectional attention, GeGLU) on the tcgen05 GEMMs and the head_dim-64 attention kernel with its
+    bidirectional attention, GeGLU) on the wgmma GEMMs and the head_dim-64 attention kernel with its
     sliding-window variant; ``token_type_ids`` unused."""
 
     _DESC = staticmethod(W.modernbert_desc)

@@ -14,7 +14,7 @@ BERT (``B2E_ARCH_BERT``), 5 + 12*L device tensors:
 
 Names on the right are HF ``BertModel`` state-dict keys (transformers/models/bert/modeling_bert.py).
 Matrices keep nn.Linear's [out_features, in_features] layout, which is the K-major B operand the
-tcgen05 GEMM wants, so no transposes are needed.
+wgmma GEMM wants, so no transposes are needed.
 """
 
 from __future__ import annotations

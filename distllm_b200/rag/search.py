@@ -70,7 +70,7 @@ class ExactIndex:
             embeddings = np.asarray(dataset['embeddings'], dtype=np.float32)
             self.dataset = dataset
         if not torch.cuda.is_available():
-            raise _native.NativeError('no CUDA device: the exact index has no CPU fallback (sm_100a only)')
+            raise _native.NativeError('no CUDA device: the exact index has no CPU fallback (sm_90a only)')
         dev = torch.device(device) if device is not None else torch.device('cuda', torch.cuda.current_device())
         matrix = torch.as_tensor(embeddings)
         if matrix.ndim != 2:

@@ -1,4 +1,4 @@
-/* b2e.h -- C ABI of libb2e.so, the B200-native embedding hot path for distllm.
+/* b2e.h -- C ABI of libb2e.so, the H100-native embedding hot path for distllm.
  *
  * Every entry point is plain C: caller-owned pointers and sizes, no C++/torch types, no exceptions.
  * Functions return 0 on success or a B2E_ERR_* code; b2e_last_error() gives the thread-local
@@ -42,7 +42,7 @@ enum {
   B2E_ERR_INVALID = 1,      /* bad argument / unsupported shape */
   B2E_ERR_CUDA = 2,         /* a CUDA runtime or driver call failed */
   B2E_ERR_UNSUPPORTED = 3,  /* architecture or feature not built yet */
-  B2E_ERR_NO_DEVICE = 4     /* no sm_100 device: there is no CPU fallback */
+  B2E_ERR_NO_DEVICE = 4     /* no sm_90 device: there is no CPU fallback */
 };
 
 enum { B2E_ARCH_BERT = 0, B2E_ARCH_ESM2 = 1, B2E_ARCH_MISTRAL = 2, B2E_ARCH_MODERNBERT = 3 };
@@ -86,7 +86,8 @@ int b2e_version(void);
  * -DB2E_STORAGE_BF16): the type of every weight matrix handed to b2e_encoder_create, of every 16-bit
  * activation and of the operands of the building-block entry points.  Both feed the tensor cores at the same
  * rate; half keeps 11 significand bits (a 32-layer Mistral-shaped model stays within 1e-3 cosine of fp32 only
- * with it), bfloat16 draws less power under the 1 kW cap (BERT / ESM-2 depths are within 5e-5 with it).  The
+ * with it), bfloat16 suffices for the BERT / ESM-2 depths (bench.py's extra.storage_ab times the same GEMM in both
+ * builds).  The
  * reference's own reduced precision is half (distllm/embed/encoders/auto.py:77-79). */
 int b2e_storage_dtype(void);
 const char* b2e_last_error(void);

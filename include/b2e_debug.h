@@ -1,9 +1,8 @@
 /* b2e_debug.h -- profiling / experiment hooks of libb2e.so.
  *
  * NOT part of the reference-facing ABI (include/b2e.h): nothing in distllm would bind these.  They
- * exist for the timeline tools under tools/ (att3_timeline.py, gemm_timeline.py, pair_experiments.py)
- * and are declared here so that every symbol the shared library exports is declared in a header.
- * All of them write a __device__ global of the kernels' translation unit; 0 on success.
+ * exist for the tests and the tools under tools/ and are declared here so that every symbol the shared
+ * library exports is declared in a header.  0 on success.
  */
 #ifndef B2E_DEBUG_H_
 #define B2E_DEBUG_H_
@@ -17,25 +16,21 @@ struct B2EEncoder;
  * drift report (tools/drift_report.py) compares every depth with the CPU oracle */
 int b2e_debug_set_layers(struct B2EEncoder* enc, int n_layers);
 
-/* device buffer of 4 x 512 int64: CTA 0 of the streaming attention kernels records (clock64, event
- * code) pairs per role (softmax slot A/B, MMA issuer, loader); NULL switches it off */
+/* device buffer of 4 x 512 int64: CTA (0, 0, 0) of a timeline instantiation of the attention kernel (variant bit 8)
+ * records (clock64, event code) pairs of its first consumer warpgroup; NULL switches it off */
 int b2e_debug_set_att3_clock(void* device_buffer);
-/* scheduling experiments of the attention kernels (attention3.cuh g_att3_flags): bits 0-1 ordering of the two
- * softmax warpgroups (0 free-running, 1 strict ping-pong, 2 de-phased once per item = default), bit 2 the loader
- * and MMA-issuer threads wait parked in hardware (mbarrier.try_wait with a suspend-time hint) instead of polling */
-int b2e_debug_set_att3_flags(int flags);
+/* which instantiated variant of the head_dim-64 attention kernel the next launches use (also B2E_ATT3; -1 = the
+ * environment / built-in default) */
+int b2e_debug_set_att3_variant(int variant);
+/* device buffer of 4 x 256 int64 filled with clock64() stamps by CTA (0, 0) of the bias GEMM while set (the
+ * timeline instantiation runs instead of the production one); NULL switches it off */
+int b2e_debug_set_clock_buffer(void* device_buffer);
 /* 0: keep the padded [B, S] token layout on every path; 1 (default, also B2E_PACKED=1): pooled forward passes run
  * on the attended tokens only (csrc/pack.cuh).  Drops the handle's cached CUDA graphs' validity: call it before
  * b2e_embed_host, not between its batches. */
 int b2e_debug_set_packing(int on);
 /* *out = 1 when this thread's last b2e_topk_ip_tc call had to fall back to the exact scan (synchronises the device) */
 int b2e_debug_topk_tc_fell_back(int* out);
-/* which instantiated softmax variant of attention3_d64_kernel<V> the next launches use (also B2E_ATT3) */
-int b2e_debug_set_att3_variant(int variant);
-/* CTA-pair GEMM: bit 0 = skip the epilogue's math and stores (experiment) */
-int b2e_debug_set_pair_flags(int flags);
-/* device buffer of 4 x 256 int64 filled with clock64() stamps by CTAs 0/1 of the CTA-pair GEMM */
-int b2e_debug_set_clock_buffer(void* device_buffer);
 
 #ifdef __cplusplus
 }

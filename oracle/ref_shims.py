@@ -2,10 +2,11 @@
 
 The reference is pure Python.  Where it comes from:
 
-  * ``baseline/_ref``   the offline ``pip install --no-deps --target baseline/_ref`` of ``/root/reference``
-                        (git-ignored, travels to the GPU box with the snapshot; made by
-                        ``__graft_entry__.build()`` in the authoring container)
-  * ``/root/reference`` the read-only tree itself (authoring container only)
+  * ``oracle/_ref``   a copy of its ``distllm`` package (git-ignored), made by ``install_reference()``
+                      (called from ``__graft_entry__.build()``) from the checkout at ``DEFAULT_SOURCE`` or the
+                      one the environment variable ``DISTLLM_REFERENCE`` names.  It travels with the tree; where
+                      neither it nor a checkout exists, the CPU arm of ``bench.py`` runs the oracle port and
+                      says so (kind "port")
 
 Two of its import-time dependencies are absent from this image and are replaced by the smallest
 stand-ins that let ``distllm.distributed_embedding.embedding_worker`` run (SURVEY 8c):
@@ -31,7 +32,9 @@ import types
 from pathlib import Path
 
 REPO = Path(__file__).resolve().parents[1]
-CANDIDATES = (REPO / 'baseline' / '_ref', Path('/root/reference'))
+TARGET = REPO / 'oracle' / '_ref'
+DEFAULT_SOURCE = Path('/root/reference')   # the unmodified ramanathanlab/distllm checkout
+CANDIDATES = (TARGET,)
 
 _BOUNDARY = re.compile(r'[.!?]["\')\]]*\s+(?=[A-Z0-9"\'(\[])')
 
@@ -42,6 +45,25 @@ def reference_root() -> Path | None:
         if (root / 'distllm' / 'distributed_embedding.py').exists():
             return root
     return None
+
+
+def install_reference() -> str:
+    """Copy the pure-Python ``distllm`` package of the reference checkout (``DISTLLM_REFERENCE``, else
+    ``DEFAULT_SOURCE``) into ``oracle/_ref`` (nothing to compile; its missing dependencies are stubbed at run
+    time, see above)."""
+    import os
+    import shutil
+
+    if reference_root() is not None:
+        return f'present: {TARGET}'
+    src = Path(os.environ.get('DISTLLM_REFERENCE') or DEFAULT_SOURCE)
+    if not (src / 'distllm' / 'distributed_embedding.py').exists():
+        return f'absent (no reference checkout at {src}); the CPU arm falls back to the oracle port'
+    tmp = TARGET.with_name(TARGET.name + '.tmp')
+    shutil.rmtree(tmp, ignore_errors=True)
+    shutil.copytree(src / 'distllm', tmp / 'distllm', ignore=shutil.ignore_patterns('__pycache__'))
+    tmp.rename(TARGET)
+    return f'installed: {TARGET}'
 
 
 def _regex_spans(text: str) -> list[tuple[int, int]]:
@@ -112,7 +134,7 @@ def install(root: Path | None = None) -> Path:
     """Make ``import distllm`` resolve to the unmodified reference; returns the root used."""
     root = root or reference_root()
     if root is None:
-        raise RuntimeError('the reference is not available: neither baseline/_ref nor /root/reference')
+        raise RuntimeError('the reference is not available: oracle/_ref is absent (run build() where a checkout exists)')
     if str(root) not in sys.path:
         sys.path.insert(0, str(root))
     _stub_parsl()

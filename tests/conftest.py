@@ -1,4 +1,4 @@
-"""Shared fixtures.  ``-m gpu`` tests need a B200; everything else runs on CPU."""
+"""Shared fixtures.  ``-m gpu`` tests need an H100; everything else runs on CPU."""
 
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ GOLDEN = REPO / 'tests' / 'golden'
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA sm_100 device (run with -m gpu on a B200)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA sm_90 device (run with -m gpu on an H100)')
 
 
 @pytest.fixture(scope='session', autouse=True)

@@ -67,10 +67,10 @@ def test_gemm_rejects_bad_shapes(dev, h16):
 
 @pytest.fixture(params=[None, 5, 0, 69, 64, 193], ids=['shipping', 'two-wg-poly', 'two-wg', 'four-wg-poly', 'four-wg-vote', 'four-wg-epilogue-role'])
 def att_variant(request, h16):
-    """Which head_dim-64 attention kernel the calls of a test reach: the library's default (variant 65: four
-    softmax warpgroups, attention5.cuh), the two-warpgroup kernel of attention3.cuh (5, 0), or the other
-    four-warpgroup flavours (69: polynomial exponentials, 64: vote over the bias row, 193: a fifth warpgroup takes
-    the per-tile epilogue)."""
+    """Which variant of the head_dim-64 attention kernel (attention.cuh) the calls of a test reach: the library's
+    default, two consumer warpgroups per CTA (5: one exponential in four as a polynomial, 0: every chunk reads its
+    bias row, none is known from attn_prep to be fully attended), or four (69: polynomial exponentials, 64: every
+    chunk reads its bias row, 193: the producer warp stores the output tiles with TMA)."""
     import ctypes
 
     lib = nv.load(nv.storage_of(h16))
@@ -123,7 +123,7 @@ def test_attention_mask_with_holes_and_fully_masked_row(dev, h16, att_variant):
 
 
 def test_attention_many_items_per_cta(dev, h16, att_variant):
-    """More work items than SMs: the persistent CTAs recycle Q buffers, ring stages and TMEM slots."""
+    """More work items than SMs: several waves of CTAs over ragged sequences, the K/V ring reused per CTA."""
     b, s, heads = 40, 300, 12
     g = torch.Generator(device=dev).manual_seed(77)
     qkv = torch.randn(b * s, 3 * heads * 64, device=dev, generator=g).to(h16)
@@ -537,7 +537,7 @@ def test_attention_d64_sliding_window(dev, b, s, heads, window, h16, att_variant
 
 # ------------------------------------------------------------------------- profiling instantiations
 def test_profiling_instantiations_write_timelines_and_change_no_result(dev):
-    """The clock64 timelines live in separate instantiations (attention: variant bit 8; pair GEMM: selected while a
+    """The clock64 timelines live in separate instantiations (attention: variant bit 8; bias GEMM: selected while a
     clock buffer is set): they must fill their buffers and give the production kernels' results bit for bit."""
     import ctypes
 
@@ -567,7 +567,7 @@ def test_profiling_instantiations_write_timelines_and_change_no_result(dev):
     finally:
         lib.b2e_debug_set_att3_clock(None)
         lib.b2e_debug_set_att3_variant(-1)
-    # pair GEMM
+    # bias GEMM
     a = (torch.randn(4096, 768, device=dev, generator=g) * 0.5).to(torch.bfloat16)
     w = (torch.randn(768, 768, device=dev, generator=g) * 0.05).to(torch.bfloat16)
     bias = torch.randn(768, device=dev, generator=g)

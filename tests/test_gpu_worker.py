@@ -1,9 +1,9 @@
-"""-m gpu: the plugin-level entry points on a B200, from files on disk to files on disk.
+"""-m gpu: the plugin-level entry points on an H100, from files on disk to files on disk.
 
 W1 `embedding_worker`, E1 `get_encoder({'name': 'auto' | 'esm2', ...}, register=True)` on local HF checkpoint
 directories (``save_pretrained``), the typer CLI and the torchrun driver -- compared with the outputs the
 UNMODIFIED reference produced for the same checkpoints and texts (tests/golden/*.npz, written by
-oracle/make_golden.py from /root/reference).
+oracle/make_golden.py from an upstream distllm checkout).
 """
 
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""BASELINE config C1 on one B200: BERT-base shape, mean pooler, batch_size=8, 1000 chunks of 128 tokens,
+"""BASELINE config C1 on one H100: BERT-base shape, mean pooler, batch_size=8, 1000 chunks of 128 tokens,
 through the host-buffer C-ABI call (b2e_embed_host: H2D + 91 launches + D2H per batch of 8).
 The small-batch regime is launch-bound; the number is reported for completeness next to C2.
 usage: bench_c1.py [batch] [seq] [n_chunks]"""

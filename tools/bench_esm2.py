@@ -1,4 +1,4 @@
-"""ESM2-650M-shape throughput on one B200 (BASELINE config C5: 1024 residues -> S=1026, mean pooler).
+"""ESM2-650M-shape throughput on one H100 (BASELINE config C5: 1024 residues -> S=1026, mean pooler).
 Synthetic ids, seeded random weights.  Prints sequences/s and the fraction of the bf16 roofline."""
 import json, sys, time
 from pathlib import Path

@@ -1,4 +1,4 @@
-"""Mistral-7B-shape throughput on one B200 (BASELINE config C3: SFR-Embedding-Mistral shape, L=32,
+"""Mistral-7B-shape throughput on one H100 (BASELINE config C3: SFR-Embedding-Mistral shape, L=32,
 H=4096, 32 query / 8 kv heads x 128, I=14336, last_token pooler, B=16, S=4096).
 Synthetic ids, seeded random bf16 weights.  Prints sequences/s, the fraction of the bf16 roofline
 (causal-skipped FLOPs, SURVEY 8d) and a per-kernel breakdown of one layer timed with CUDA events.
@@ -49,7 +49,7 @@ flops_causal = L * (2.0 * S * H * QC + 2.0 * S * H * H + 6.0 * S * H * I + 2.0 *
 seqs = B / (ms * 1e-3)
 pk = Path(__file__).resolve().parents[1] / 'MEASURED_PEAKS.json'
 peaks = json.loads(pk.read_text()) if pk.exists() else {}
-sus = peaks.get('bf16_tflops_sustained', 1415.2)
+sus = peaks.get('bf16_tflops_sustained', 989.0)   # H100 SXM data sheet, dense 16-bit
 res = {'workload': f'C3: Mistral-7B shape (L={L}), S={S}, last_token pooler' + (' RAGGED' if RAGGED else ''), 'batch': B,
        'attended_tokens': int(mask.sum().item()), 'padded_tokens': B * S, 'ms_per_step': ms,
        'sequences_per_s': seqs, 'tflops_causal_skipped': seqs * flops_causal / 1e12,

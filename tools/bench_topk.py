@@ -12,7 +12,7 @@ N = int(sys.argv[1]) if len(sys.argv) > 1 else 2_000_000
 H = int(sys.argv[2]) if len(sys.argv) > 2 else 768
 dev = torch.device('cuda:0')
 pk = Path(__file__).resolve().parents[1] / 'MEASURED_PEAKS.json'
-hbm = json.loads(pk.read_text()).get('hbm_gbs', 6570.3) if pk.exists() else 6570.3
+hbm = json.loads(pk.read_text()).get('hbm_gbs', 3350.0) if pk.exists() else 3350.0   # H100 SXM data sheet
 g = torch.Generator(device=dev).manual_seed(0)
 for dtype in (torch.float32, torch.bfloat16):
     corpus = torch.randn(N, H, device=dev, generator=g)

@@ -1,4 +1,4 @@
-"""End-to-end `embedding_worker` on one B200 with the HOST FEED included: synthetic jsonl documents ->
+"""End-to-end `embedding_worker` on one H100 with the HOST FEED included: synthetic jsonl documents ->
 sentence split -> buffers -> HF fast tokenizer in DataLoader workers -> native encoder -> semantic
 chunking -> second pass -> numpy writer (SURVEY 8(f) rank 1: where does the time go once the encoder
 runs near the roofline?).  BERT-base shape, seeded random weights saved as a local HF checkpoint.

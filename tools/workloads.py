@@ -119,8 +119,7 @@ def add_outliers(state_dict: dict, family: str, seed: int = 0, n_massive: int = 
 
     (A first version drew EVERY gain from [0.1, 10]: with all q/k inputs up to 10x larger the attention
     logits grow ~100x, softmax turns into an arg-max, and the fp32 network itself becomes discontinuous in
-    its inputs -- any 16-bit implementation then flips keys at random tokens.  profiles/r02_drift_report.md
-    keeps that run as the documented stress case.)"""
+    its inputs -- any 16-bit implementation then flips keys at random tokens.)"""
     g = torch.Generator().manual_seed(seed)
     out_names = _OUT_ROWS[family]
     hidden = next(v.shape[0] for k, v in state_dict.items() if k.endswith(out_names[0]))
