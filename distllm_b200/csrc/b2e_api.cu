@@ -184,11 +184,18 @@ int launch_gemm_epi(const CUtensorMap& ta, const CUtensorMap& tb, void* out, con
   auto kern = gemm_h16_wgmma_kernel<EPI>;
   if constexpr (EPI == EPI_BIAS)
     if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true>;
-  const int arc = ensure_smem_attr(kern, GEMM_SMEM_BYTES);
-  if (arc) return arc;
+  int rc = ensure_smem_attr(kern, GEMM_SMEM_BYTES);
+  if (rc) return rc;
+  DeviceInfo dev;
+  if ((rc = current_device_info(&dev))) return rc;
   const long long tiles = (long long)(N / GEMM_BN) * ((M + GEMM_BM - 1) / GEMM_BM);
   if (tiles > 0x7fffffffLL) return fail(B2E_ERR_INVALID, "gemm: %lld output tiles exceed one grid", tiles);
-  kern<<<(unsigned)tiles, GEMM_THREADS, GEMM_SMEM_BYTES, st>>>(ta, tb, static_cast<h16*>(out), bias, resid, M, N, K, m_dev);
+  CUtensorMap tm_out;   // the epilogue's TMA stores: 64-column boxes of 128 rows
+  if ((rc = make_tmap_h16(&tm_out, out, M, epi_is_glu(EPI) ? N / 2 : N, GEMM_BM))) return rc;
+  // persistent: one CTA per SM (fewer for small problems), each walking its share of the tiles
+  const unsigned grid = (unsigned)(tiles < dev.sms ? tiles : dev.sms);
+  kern<<<grid, GEMM_THREADS, GEMM_SMEM_BYTES, st>>>(ta, tb, tm_out, static_cast<h16*>(out), bias, resid, M, N, K,
+                                                    m_dev);
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
 }

@@ -1,13 +1,17 @@
-// Warp-specialised h16 GEMM for sm_90a:  out[M,N] = epi(A[M,K] . W[N,K]^T + bias)
+// Persistent, warp-specialised h16 GEMM for sm_90a:  out[M,N] = epi(A[M,K] . W[N,K]^T + bias)
 //
-//   warp 8      TMA producer (one elected lane): 128 x 64 A tile and 128 x 64 W tile per stage into a
-//               128B-swizzled shared-memory ring
-//   warps 0-7   two consumer warpgroups, 64 output rows each: wgmma m64n128k16 with both operands read
-//               from shared memory, fp32 accumulators in registers; the epilogue (+bias, erf-GELU |
-//               +residual | gated activation) runs on those registers and stores h16 pairs
+//   warpgroup 2   TMA producer (one elected lane, 40 registers): for every tile of the CTA, the 128 x 64 A box
+//                 and the 128 x 64 W box of each k-block into a five-stage 128B-swizzled shared-memory ring
+//   warpgroups    two consumers (232 registers each), each owning a whole 128 x 128 output tile: two wgmma
+//   0 and 1       m64n128k16 per k16 step sharing the W descriptor, 128 fp32 accumulators per thread; the
+//                 epilogue (+bias, erf-GELU | +residual | gated activation) runs on those registers, writes h16
+//                 pairs into the warpgroup's swizzled staging tile and one thread stores it with TMA
 //
-// One CTA per 128 x 128 output tile; three 32 KiB stages keep two CTAs resident per SM, so the epilogue
-// of one overlaps the main loop of the other.
+// One CTA per SM walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tiles fastest, so that the CTAs
+// running together share their A rows in L2); consumer 0 takes the CTA's even-numbered tiles, consumer 1 the
+// odd ones.  Ping-pong: two named barriers pass the tensor cores from one consumer to the other at the end of
+// each main loop, so the epilogue of one tile runs while the other consumer's main loop keeps the tensor cores
+// busy, and the two main loops never interleave.
 //
 // This replaces the cuBLAS nn.Linear calls HF BERT issues from
 // transformers/models/bert/modeling_bert.py:180-182 (q,k,v), :294-298 (attn out), :339-342 (FFN up +
@@ -29,13 +33,19 @@ __host__ __device__ constexpr bool epi_is_glu(int epi) { return epi == EPI_SWIGL
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BN = 128;
 constexpr int GEMM_BK = 64;  // 64 h16 = one 128-byte swizzle row
-constexpr int GEMM_STAGES = 3;
-constexpr int GEMM_THREADS = 288;   // two consumer warpgroups + the producer warp
+constexpr int GEMM_STAGES = 5;
+constexpr int GEMM_THREADS = 384;   // two consumer warpgroups + the producer warpgroup
+constexpr int GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 Ki registers
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;
 constexpr int GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_BN * GEMM_BK * 2;
-constexpr int GEMM_BAR_OFFSET = GEMM_STAGES * GEMM_STAGE_BYTES;
-constexpr int GEMM_SMEM_BYTES = GEMM_BAR_OFFSET + 64 + 1024;   // + slack to align the ring to 1024 B
-static_assert(2 * GEMM_SMEM_BYTES <= 232448, "two CTAs per SM");
+constexpr int GEMM_OUT_BOX = GEMM_BM * 64 * 2;   // one 64-column TMA store box of a tile, 16 KiB
+constexpr int GEMM_OUT_OFFSET = GEMM_STAGES * GEMM_STAGE_BYTES;   // [consumer][2 boxes] staging tiles
+constexpr int GEMM_BAR_OFFSET = GEMM_OUT_OFFSET + 2 * 2 * GEMM_OUT_BOX;
+constexpr int GEMM_SMEM_BYTES = GEMM_BAR_OFFSET + 16 * GEMM_STAGES + 1024;   // + slack to align to 1024 B
+static_assert(GEMM_SMEM_BYTES <= 232448, "shared memory of one SM");
+// named barriers: GEMM_BAR_TURN + w = consumer w may issue its main loop; GEMM_BAR_STAGE + w = consumer w's
+// staging tile is free / written
+constexpr int GEMM_BAR_TURN = 1, GEMM_BAR_STAGE = 3;
 
 // erf-GELU, x * Phi(x), with Phi from the Abramowitz-Stegun 7.1.26 erfc polynomial
 // (|erf error| <= 1.5e-7): gelu(x) = max(x,0) - 0.5*|x|*poly(t)*exp(-x^2/2), t = 1/(1 + p*|x|/sqrt2).
@@ -76,24 +86,36 @@ __device__ __forceinline__ float silu(float x) {
   return x * r;
 }
 
+
 // profiling aid (b2e_debug_set_clock_buffer): CTA 0 of the TL instantiation records clock64() once per
 // K block in the producer ([0][n], after issuing the loads) and in the first consumer warpgroup ([1][n], when
 // the block's MMAs have been retired); 4 x 256 int64
 __device__ long long* g_gemm_clock = nullptr;
 
+// The tiles of CTA blockIdx.x: first, first + stride, ... (count of them) of the linear tile index, N tiles
+// fastest, over the rows [0, M) the kernel was given.  Every role derives its sequence from here, so that the
+// producer pushes exactly the k-blocks the consumers pop and both consumers agree on whose turn is next.
+struct GemmTiles {
+  int first, stride, count, n_tiles;
+};
+__device__ __forceinline__ GemmTiles gemm_tiles(int M, int N) {
+  const int n_tiles = N / GEMM_BN;
+  const int tiles = n_tiles * ((M + GEMM_BM - 1) / GEMM_BM);
+  const int first = static_cast<int>(blockIdx.x), stride = static_cast<int>(gridDim.x);
+  return {first, stride, first < tiles ? (tiles - 1 - first) / stride + 1 : 0, n_tiles};
+}
+
 template <int EPI, bool TL = false>
-__global__ void __launch_bounds__(GEMM_THREADS, 2)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
                       const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x 128
+                      const __grid_constant__ CUtensorMap tm_out,  // out [M,N] (GLU: [M,N/2]) box 64 x 128
                       h16* __restrict__ out, const float* __restrict__ bias, const h16* __restrict__ resid,
                       int M, int N, int K, const int* __restrict__ m_dev) {
   if (m_dev != nullptr) M = __ldg(m_dev);   // device-resident row count (packed token layout)
-  // one-dimensional grid, N tiles fastest: the CTAs resident together share their A rows in L2
-  const int n_blk = static_cast<int>(blockIdx.x % (N / GEMM_BN)), m_blk = static_cast<int>(blockIdx.x / (N / GEMM_BN));
-  if (m_blk * GEMM_BM >= M) return;
+  const GemmTiles tl = gemm_tiles(M, N);
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t sb = (raw + 1023u) & ~1023u;   // the swizzled tiles need a 1024-byte aligned base
+  const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;   // the swizzled tiles need a 1024-byte aligned base
   const uint32_t full_bar = sb + GEMM_BAR_OFFSET;
   const uint32_t empty_bar = full_bar + 8u * GEMM_STAGES;
   const int warp = threadIdx.x >> 5;
@@ -102,111 +124,175 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   if (threadIdx.x == 0) {
     for (int s = 0; s < GEMM_STAGES; ++s) {
       mbar_init(full_bar + 8u * s, 1);
-      mbar_init(empty_bar + 8u * s, 2);   // one arrival per consumer warpgroup
+      mbar_init(empty_bar + 8u * s, 1);   // released by the one consumer whose tile the k-block belongs to
     }
     mbar_fence_init();
   }
   __syncthreads();
 
   long long* clk = (TL && blockIdx.x == 0) ? g_gemm_clock : nullptr;
-  if (warp == 8) {
-    if (elect_one()) {
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GEMM_PRODUCER_REGS));
+    if (warp == 8 && elect_one()) {
       tma_prefetch_desc(&tm_a);
       tma_prefetch_desc(&tm_b);
-      int stage = 0;
+      int stage = 0, n = 0;
       uint32_t phase = 0;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
-        const uint32_t dst = sb + stage * GEMM_STAGE_BYTES;
-        const uint32_t fb = full_bar + 8u * stage;
-        mbar_expect_tx(fb, GEMM_STAGE_BYTES);
-        tma_load_2d(dst, &tm_a, fb, kb * GEMM_BK, m_blk * GEMM_BM);
-        tma_load_2d(dst + GEMM_A_BYTES, &tm_b, fb, kb * GEMM_BK, n_blk * GEMM_BN);
-        if (TL && clk != nullptr && kb < 256) clk[kb] = clock64();
-        if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
+      for (int i = 0; i < tl.count; ++i) {
+        const int tile = tl.first + i * tl.stride;
+        const int m0 = (tile / tl.n_tiles) * GEMM_BM, n0 = (tile % tl.n_tiles) * GEMM_BN;
+        for (int kb = 0; kb < kblocks; ++kb, ++n) {
+          mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
+          const uint32_t dst = sb + stage * GEMM_STAGE_BYTES;
+          const uint32_t fb = full_bar + 8u * stage;
+          mbar_expect_tx(fb, GEMM_STAGE_BYTES);
+          tma_load_2d(dst, &tm_a, fb, kb * GEMM_BK, m0);
+          tma_load_2d(dst + GEMM_A_BYTES, &tm_b, fb, kb * GEMM_BK, n0);
+          if (TL && clk != nullptr && n < 256) clk[n] = clock64();
+          if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
+        }
       }
     }
     return;
   }
 
-  const int wg = warp >> 2;                  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(GEMM_CONSUMER_REGS));
+  const int wg = warp >> 2;
   const int t = threadIdx.x & 127;
-  float acc[64];
+  const int quad = t & 3;
+  const int r_lo = 16 * (t >> 5) + ((t & 31) >> 2);   // row of acc[h][4j + {0,1}] in its 64-row half
+  const uint32_t stg = sb + GEMM_OUT_OFFSET + wg * (2 * GEMM_OUT_BOX);
+  int retired = 0;
+  // Turn i (the CTA's i-th tile) belongs to consumer i % 2.  The hand-over into turn i (1 <= i < count) is one
+  // arrive by the consumer of turn i - 1 after issuing its main loop and one sync by the consumer of turn i
+  // before starting its own: every arrive has its sync, and with 0 or 1 tiles nobody waits.
+  for (int i = wg; i < tl.count; i += 2) {
+    const int tile = tl.first + i * tl.stride;
+    const int m0 = (tile / tl.n_tiles) * GEMM_BM, n_blk = tile % tl.n_tiles;
+    float acc[2][64];   // rows [64 h, 64 h + 64) of the tile
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
-  int stage = 0;
-  uint32_t phase = 0;
-  int prev = -1;
-  for (int kb = 0; kb < kblocks; ++kb) {
-    mbar_wait(full_bar + 8u * stage, phase);
-    const uint32_t a_addr = sb + stage * GEMM_STAGE_BYTES + wg * (64 * 128);
-    const uint64_t a_desc = make_smem_desc_sw128(a_addr);
-    const uint64_t b_desc = make_smem_desc_sw128(sb + stage * GEMM_STAGE_BYTES + GEMM_A_BYTES);
-    reg_fence(acc);
-    wgmma_fence();
+    for (int x = 0; x < 64; ++x) acc[0][x] = acc[1][x] = 0.0f;
+    if (i > 0) named_bar_sync(GEMM_BAR_TURN + wg, 256);
+    // this tile's k-blocks follow the i * kblocks ones of the earlier turns in the ring
+    const int it = i * kblocks;
+    int stage = it % GEMM_STAGES;
+    uint32_t phase = (it / GEMM_STAGES) & 1u;
+    int prev = -1;
+    for (int kb = 0; kb < kblocks; ++kb) {
+      mbar_wait(full_bar + 8u * stage, phase);
+      const uint32_t a_addr = sb + stage * GEMM_STAGE_BYTES;
+      const uint64_t a0 = make_smem_desc_sw128(a_addr), a1 = make_smem_desc_sw128(a_addr + 64 * 128);
+      const uint64_t b_desc = make_smem_desc_sw128(a_addr + GEMM_A_BYTES);
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_64x128_ss(acc, a_desc + 2u * k, b_desc + 2u * k, (kb | k) != 0);
-    wgmma_commit();
-    reg_fence(acc);
-    // keep one stage of MMAs in flight: the previous one has finished reading its operands
-    wgmma_wait<1>();
-    reg_fence(acc);
-    if (prev >= 0 && t == 0) mbar_arrive(empty_bar + 8u * prev);
-    if (TL && clk != nullptr && threadIdx.x == 0 && kb < 256) clk[256 + kb] = clock64();
-    prev = stage;
-    if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
-  }
-  wgmma_wait<0>();
-  reg_fence(acc);
+      for (int k = 0; k < GEMM_BK / 16; ++k) {
+        wgmma_64x128_ss(acc[0], a0 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+        wgmma_64x128_ss(acc[1], a1 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+      }
+      wgmma_commit();
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      // keep one stage of MMAs in flight: the previous one has finished reading its operands
+      wgmma_wait<1>();
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      if (prev >= 0 && t == 0) mbar_arrive(empty_bar + 8u * prev);
+      if (TL && clk != nullptr && wg == 0 && t == 0 && retired < 256) clk[256 + retired] = clock64();
+      ++retired;
+      prev = stage;
+      if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
+    }
+    if (i + 1 < tl.count) named_bar_arrive(GEMM_BAR_TURN + (wg ^ 1), 256);   // the other consumer's turn
+    wgmma_wait<0>();
+    reg_fence(acc[0]);
+    reg_fence(acc[1]);
+    if (t == 0) mbar_arrive(empty_bar + 8u * prev);
 
-  const int r_lo = m_blk * GEMM_BM + wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
-  const int c_in = 2 * (t & 3);
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    const int row = r_lo + 8 * half;
-    if (row >= M) continue;
+    // Epilogue.  A tile inside the device rows goes out through the staging tile (128-byte swizzle, the
+    // layout of the store map: 16-byte unit u of row r sits at unit u ^ (r & 7), so that the eight rows of a
+    // warp's store hit distinct banks) and TMA; a tile crossing M stores its rows from registers.
+    const bool staged = m0 + GEMM_BM <= M;
+    if (staged) {
+      if (t == 0) tma_store_wait_read<0>();   // the previous tile's stores have read the staging tile
+      named_bar_sync(GEMM_BAR_STAGE + wg, 128);
+    }
     if constexpr (epi_is_glu(EPI)) {
       const int n_out = N / 2;
-      h16* orow = out + static_cast<size_t>(row) * n_out + n_blk * (GEMM_BN / 2);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float g0 = acc[4 * j + 2 * half], g1 = acc[4 * j + 2 * half + 1];
-        const float u0 = acc[4 * (j + 8) + 2 * half], u1 = acc[4 * (j + 8) + 2 * half + 1];
-        float v0, v1;
-        if (EPI == EPI_GEGLU) {
-          v0 = gelu_erf_fast(g0) * u0;
-          v1 = gelu_erf_fast(g1) * u1;
-        } else {
-          v0 = silu(g0) * u0;
-          v1 = silu(g1) * u1;
-        }
-        *reinterpret_cast<uint32_t*>(orow + 8 * j + c_in) = pack_h16x2(v0, v1);
-      }
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int r = 64 * h + r_lo + 8 * half;
+            const float g0 = acc[h][4 * j + 2 * half], g1 = acc[h][4 * j + 2 * half + 1];
+            const float u0 = acc[h][4 * (j + 8) + 2 * half], u1 = acc[h][4 * (j + 8) + 2 * half + 1];
+            float v0, v1;
+            if (EPI == EPI_GEGLU) {
+              v0 = gelu_erf_fast(g0) * u0;
+              v1 = gelu_erf_fast(g1) * u1;
+            } else {
+              v0 = silu(g0) * u0;
+              v1 = silu(g1) * u1;
+            }
+            if (staged)
+              st_shared_u32(stg + r * 128 + ((j ^ (r & 7)) << 4) + 4 * quad, pack_h16x2(v0, v1));
+            else if (m0 + r < M)
+              *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(m0 + r) * n_out + n_blk * (GEMM_BN / 2) +
+                                           8 * j + 2 * quad) = pack_h16x2(v0, v1);
+          }
     } else {
-      const int col0 = n_blk * GEMM_BN + c_in;
-      h16* orow = out + static_cast<size_t>(row) * N + col0;
-      const h16* rrow = (EPI == EPI_BIAS_RESID) ? resid + static_cast<size_t>(row) * N + col0 : nullptr;
+      const int col0 = n_blk * GEMM_BN + 2 * quad;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
-        if (bias != nullptr) {
-          const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * j));
-          v0 += b.x;
-          v1 += b.y;
+        const float2 b = bias != nullptr ? __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * j))
+                                         : make_float2(0.0f, 0.0f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int r = 64 * h + r_lo + 8 * half;
+            if (!staged && m0 + r >= M) continue;
+            float v0 = acc[h][4 * j + 2 * half], v1 = acc[h][4 * j + 2 * half + 1];
+            if (bias != nullptr) {
+              v0 += b.x;
+              v1 += b.y;
+            }
+            if (EPI == EPI_BIAS_GELU) {
+              v0 = gelu_erf_fast(v0);
+              v1 = gelu_erf_fast(v1);
+            }
+            const size_t off = static_cast<size_t>(m0 + r) * N + col0 + 8 * j;
+            if (EPI == EPI_BIAS_RESID) {
+              const float2 rv = unpack_h16x2(*reinterpret_cast<const uint32_t*>(resid + off));
+              v0 += rv.x;
+              v1 += rv.y;
+            }
+            if (staged)
+              st_shared_u32(stg + (j >> 3) * GEMM_OUT_BOX + r * 128 + (((j & 7) ^ (r & 7)) << 4) + 4 * quad,
+                            pack_h16x2(v0, v1));
+            else
+              *reinterpret_cast<uint32_t*>(out + off) = pack_h16x2(v0, v1);
+          }
+      }
+    }
+    if (staged) {
+      fence_proxy_async_smem();   // the staging tile is read by the TMA (async proxy)
+      named_bar_sync(GEMM_BAR_STAGE + wg, 128);
+      if (t == 0) {
+        if constexpr (epi_is_glu(EPI)) {
+          tma_store_2d(&tm_out, stg, n_blk * (GEMM_BN / 2), m0);
+        } else {
+          tma_store_2d(&tm_out, stg, n_blk * GEMM_BN, m0);
+          tma_store_2d(&tm_out, stg + GEMM_OUT_BOX, n_blk * GEMM_BN + 64, m0);
         }
-        if (EPI == EPI_BIAS_GELU) {
-          v0 = gelu_erf_fast(v0);
-          v1 = gelu_erf_fast(v1);
-        }
-        if (EPI == EPI_BIAS_RESID) {
-          const float2 r = unpack_h16x2(*reinterpret_cast<const uint32_t*>(rrow + 8 * j));
-          v0 += r.x;
-          v1 += r.y;
-        }
-        *reinterpret_cast<uint32_t*>(orow + 8 * j) = pack_h16x2(v0, v1);
+        tma_store_commit();
       }
     }
   }
+  if (t == 0) tma_store_wait_all();   // the stores have read shared memory before the CTA leaves
 }
 
 }  // namespace b2e
