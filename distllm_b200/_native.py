@@ -69,6 +69,7 @@ EXPORTS = (
     'b2e_adjacent_cosine_dist',
     'b2e_gemm_h16',
     'b2e_attention_d64',
+    'b2e_attention_d32',
     'b2e_attention_d64_window',
     'b2e_attention_causal_d128',
     'b2e_topk_ip',
@@ -155,6 +156,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_gemm_h16.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b2e_attention_d64.restype = i32
     lib.b2e_attention_d64.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
+    lib.b2e_attention_d32.restype = i32
+    lib.b2e_attention_d32.argtypes = [vp, vp, vp, i32, i32, i32, vp]
     lib.b2e_attention_d64_window.restype = i32
     lib.b2e_attention_d64_window.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b2e_attention_causal_d128.restype = i32
@@ -269,6 +272,17 @@ def attention_d64(
     with torch.cuda.device(qkv.device):
         check(lib.b2e_attention_d64(qkv.data_ptr(), attention_mask.data_ptr(), ctx.data_ptr(), batch,
                                     seq, heads, None, stream_ptr(qkv.device)), lib)
+    return ctx
+
+
+def attention_d32(qkv: torch.Tensor, attention_mask: torch.Tensor, batch: int, seq: int, heads: int) -> torch.Tensor:
+    """Head_dim-32 attention (MiniLM / BGE-small / E5-small, ESM-2 150M): qkv [B*S, 3*heads*32] -> [B*S, heads*32]."""
+    lib = load(storage_of(qkv.dtype))
+    _cuda_contig(qkv, 'qkv'), _cuda_contig(attention_mask, 'attention_mask')
+    ctx = torch.zeros((batch * seq, heads * 32), dtype=qkv.dtype, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        check(lib.b2e_attention_d32(qkv.data_ptr(), attention_mask.data_ptr(), ctx.data_ptr(), batch, seq, heads,
+                                    stream_ptr(qkv.device)), lib)
     return ctx
 
 

@@ -1,13 +1,14 @@
-// Streaming self-attention for sm_90a, head_dim 64 or 128, any S.
+// Streaming self-attention for sm_90a, head_dim 32, 64 or 128, any S.
 //
 // One CTA per (query tile of 128 rows, head, sequence); two consumer warpgroups own 64 query rows each and
 // one producer warp streams the head's K/V through a shared-memory ring in 64-key chunks with TMA, so S is
 // not limited by shared memory.  Per chunk and warpgroup:
 //
-//   S_j = Q K_j^T       wgmma m64n64k16, Q and K_j both K-major (128B-swizzled TMA boxes) in shared memory
+//   S_j = Q K_j^T       wgmma m64n64k16, Q and K_j both K-major (128B-swizzled TMA boxes of 64 columns; at head_dim
+//                       32 one 64B-swizzled box of 32 columns) in shared memory
 //   online softmax      in registers, exp2 domain; every row's 64 scores live in the 4 lanes of a quad
-//   O  += P_j V_j       wgmma m64n64k16 per 64 output columns, P_j from registers (the S accumulator
-//                       layout IS the A fragment layout), V_j as an MN-major shared-memory operand
+//   O  += P_j V_j       wgmma m64n64k16 per 64 output columns (m64n32k16 at head_dim 32), P_j from registers (the
+//                       S accumulator layout IS the A fragment layout), V_j as an MN-major shared-memory operand
 //
 // MODE 0  bidirectional attention with the additive key-padding bias (HF SDPA with an additive mask:
 //         transformers/models/bert/modeling_bert.py:192-205, :692-716; the same call pattern serves ESM's).
@@ -35,12 +36,16 @@
 namespace b2e {
 
 constexpr int AT_KC = 64;                  // keys per chunk
-constexpr int AT_BOX = 64 * 64 * 2;        // one TMA box: 64 rows x 64 h16 columns, 8 KiB
 constexpr float AT_MASKED = -3.0e38f;
 
 template <int D, int V>
 struct AtCfg {
-  static constexpr int NB = D / 64;                        // 64-column boxes per row of Q / K / V
+  // one TMA box: 64 rows of one swizzle row each -- 64 h16 columns (128 B, 128-byte swizzle, 8 KiB) for head_dim 64
+  // and 128, 32 columns (64 B, 64-byte swizzle, 4 KiB) for head_dim 32
+  static constexpr int COLS = D < 64 ? D : 64;
+  static constexpr int ROW_BYTES = 2 * COLS;
+  static constexpr int BOX = 64 * ROW_BYTES;
+  static constexpr int NB = D / COLS;                      // boxes per row of Q / K / V
   static constexpr int NWG = (V & 64) ? 4 : 2;             // consumer warpgroups, 64 query rows each
   static constexpr int QT = 64 * NWG;                      // query rows per CTA
   // + the producer: one warp, or with four consumer warpgroups a whole warpgroup, so that it can hand its
@@ -48,9 +53,10 @@ struct AtCfg {
   // and 112 in the consumers -- without that the 544-thread kernel is held to 96 and spills
   static constexpr int THREADS = 128 * NWG + (NWG == 4 ? 128 : 32);
   static constexpr int CONSUMER_REGS = 112, PRODUCER_REGS = 24;
-  static constexpr int STAGES = D == 64 ? 4 : 3;
-  static constexpr int Q_BYTES = NWG * NB * AT_BOX;        // [warpgroup][box]
-  static constexpr int STAGE_BYTES = 2 * NB * AT_BOX;      // K boxes | V boxes
+  static constexpr int STAGES = D == 128 ? 3 : 4;
+  static constexpr int Q_BYTES = NWG * NB * BOX;           // [warpgroup][box]
+  static constexpr int STAGE_BYTES = 2 * NB * BOX;         // K boxes | V boxes
+  static_assert(D == 32 || D == 64 || D == 128, "head_dim");
   static constexpr int BAR = Q_BYTES + STAGES * STAGE_BYTES;
   static constexpr int SMEM_BYTES = BAR + 256 + 1024;      // + slack to align the tiles to 1024 B
   static_assert(SMEM_BYTES <= 232448, "shared memory");
@@ -73,6 +79,13 @@ __device__ __forceinline__ float poly_exp2(float x) {
   p = fmaf(f, p, 6.9314718e-1f);
   p = fmaf(f, p, 1.0f);
   return __int_as_float(__float_as_int(p) + (static_cast<int>(n) << 23));
+}
+
+// shared-memory descriptor of a Q / K / V box (AtCfg::ROW_BYTES: 128- or 64-byte swizzle)
+template <int ROW_BYTES>
+__device__ __forceinline__ uint64_t at_box_desc(uint32_t saddr) {
+  if constexpr (ROW_BYTES == 128) return make_smem_desc_sw128(saddr);
+  else return make_smem_desc_sw64(saddr);
 }
 
 // bias[b, j] for j < S_pad (multiple of 64) and kv_chunks[b] = chunks holding an attended key
@@ -109,8 +122,8 @@ __global__ void attn_prep_kernel(const int64_t* __restrict__ mask, float* __rest
   }
 }
 
-// tm: the whole qkv matrix [T, (heads + 2 kv_heads) D] (columns q heads | k heads | v heads), box 64 x 64.
-// tm_ctx: ctx [T, heads D], box 64 x 64 (bit-7 variants only).  seq_cu / seq_len (nullable): token layout
+// tm: the whole qkv matrix [T, (heads + 2 kv_heads) D] (columns q heads | k heads | v heads), box 64 x AtCfg::COLS.
+// tm_ctx: ctx [T, heads D], the same box (bit-7 variants only).  seq_cu / seq_len (nullable): token layout
 // (pack.cuh), rows [row0, row0 + len) hold sequence b; the padded layout (b S, S) when null.
 template <int D, int MODE, int V>
 // one CTA per SM is what the launch bounds promise: with two the two-warpgroup kernel is held to 96 registers
@@ -123,6 +136,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
                  h16* __restrict__ ctx) {
   using Cfg = AtCfg<D, V>;
   constexpr int NB = Cfg::NB;
+  constexpr int COLS = Cfg::COLS, BOX = Cfg::BOX, RB = Cfg::ROW_BYTES;
   constexpr int NWG = Cfg::NWG;
   constexpr int POLY = (V >> 2) & 3;
   constexpr bool EPI_ROLE = (V & 128) != 0;
@@ -179,7 +193,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
       for (int w = 0; w < NWG; ++w)
 #pragma unroll
         for (int x = 0; x < NB; ++x)
-          tma_load_2d(sb + (w * NB + x) * AT_BOX, &tm, q_bar, qcol + 64 * x, row0 + q0 + 64 * w);
+          tma_load_2d(sb + (w * NB + x) * BOX, &tm, q_bar, qcol + COLS * x, row0 + q0 + 64 * w);
       int stage = 0;
       uint32_t phase = 0;
       for (int c = lo; c < hi; ++c) {
@@ -189,8 +203,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
         mbar_expect_tx(fb, Cfg::STAGE_BYTES);
 #pragma unroll
         for (int x = 0; x < NB; ++x) {
-          tma_load_2d(dst + x * AT_BOX, &tm, fb, kcol + 64 * x, row0 + c * AT_KC);
-          tma_load_2d(dst + (NB + x) * AT_BOX, &tm, fb, vcol + 64 * x, row0 + c * AT_KC);
+          tma_load_2d(dst + x * BOX, &tm, fb, kcol + COLS * x, row0 + c * AT_KC);
+          tma_load_2d(dst + (NB + x) * BOX, &tm, fb, vcol + COLS * x, row0 + c * AT_KC);
         }
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1u; }
       }
@@ -201,7 +215,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
           if (q0 + 64 * w + 64 > len) continue;   // partial tile: its warpgroup stored the rows itself
 #pragma unroll
           for (int x = 0; x < NB; ++x)
-            tma_store_2d(&tm_ctx, sb + (w * NB + x) * AT_BOX, h * D + 64 * x, row0 + q0 + 64 * w);
+            tma_store_2d(&tm_ctx, sb + (w * NB + x) * BOX, h * D + COLS * x, row0 + q0 + 64 * w);
         }
         tma_store_commit();
         tma_store_wait_all();   // the stores have read shared memory before the CTA leaves
@@ -216,16 +230,17 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
   const int quad = t & 3;
   const int qr = q0 + 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);   // query row of half 0; half 1 is qr + 8
   const float* brow = bias + static_cast<size_t>(b) * S_pad;
-  const uint32_t q_addr = sb + wg * NB * AT_BOX;
+  const uint32_t q_addr = sb + wg * NB * BOX;
   long long* clk = nullptr;
   int n_stamp = 0;
   if (STAMPS && blockIdx.x == 0 && threadIdx.x == 0) clk = g_att_clock;
 
-  float o[NB][32];
+  constexpr int OG = COLS / 8;   // 8-column groups of one box's output accumulator (m64nCOLS: 4 OG floats)
+  float o[NB][4 * OG];
 #pragma unroll
   for (int x = 0; x < NB; ++x)
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[x][i] = 0.0f;
+    for (int i = 0; i < 4 * OG; ++i) o[x][i] = 0.0f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.0f, 0.0f};
 
   mbar_wait(q_bar, 0);
@@ -234,15 +249,17 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
   for (int c = lo; c < hi; ++c) {
     mbar_wait(full_bar + 8u * stage, phase);
     const uint32_t k_addr = sb + Cfg::Q_BYTES + stage * Cfg::STAGE_BYTES;
-    const uint32_t v_addr = k_addr + NB * AT_BOX;
+    const uint32_t v_addr = k_addr + NB * BOX;
     float s[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) s[i] = 0.0f;
     wgmma_fence();
+    // k16 steps: COLS / 16 inside each box row (32 B = +2 in the descriptor's address field each), then the next box
+    constexpr int KB = COLS / 16;
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk)
-      wgmma_64x64_ss<0>(s, make_smem_desc_sw128(q_addr + (kk >> 2) * AT_BOX) + 2u * (kk & 3),
-                        make_smem_desc_sw128(k_addr + (kk >> 2) * AT_BOX) + 2u * (kk & 3), kk != 0);
+      wgmma_64x64_ss<0>(s, at_box_desc<RB>(q_addr + (kk / KB) * BOX) + 2u * (kk % KB),
+                        at_box_desc<RB>(k_addr + (kk / KB) * BOX) + 2u * (kk % KB), kk != 0);
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
@@ -300,7 +317,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
 #pragma unroll
     for (int x = 0; x < NB; ++x)
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < OG; ++j) {
         o[x][4 * j + 0] *= alpha[0];
         o[x][4 * j + 1] *= alpha[0];
         o[x][4 * j + 2] *= alpha[1];
@@ -313,8 +330,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
 #pragma unroll
     for (int kc = 0; kc < 4; ++kc)
 #pragma unroll
-      for (int x = 0; x < NB; ++x)
-        wgmma_64x64_rs_tb(o[x], p[kc], make_smem_desc_sw128(v_addr + x * AT_BOX + kc * 16 * 128));
+      for (int x = 0; x < NB; ++x) {
+        if constexpr (COLS == 64) wgmma_64x64_rs_tb(o[x], p[kc], make_smem_desc_sw128(v_addr + x * BOX + kc * 16 * 128));
+        else wgmma_64x32_rs_tb(o[x], p[kc], make_smem_desc_sw64(v_addr + x * BOX + kc * 16 * 64));
+      }
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
@@ -338,13 +357,15 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
     const float inv = 1.0f / tot;
     const int q = qr + 8 * hf;
     if (staged) {
-      const int r = q - q0 - 64 * wg;   // row inside the 64-row tile; 128-byte swizzle: unit ^= row & 7
+      // row inside the 64-row tile; 16-byte unit ^= row & 7 (128-byte swizzle) or (row >> 1) & 3 (64-byte swizzle)
+      const int r = q - q0 - 64 * wg;
+      const int swz = RB == 128 ? (r & 7) : ((r >> 1) & 3);
 #pragma unroll
       for (int x = 0; x < NB; ++x)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t off = r * 128 + ((j ^ (r & 7)) << 4) + 4 * quad;
-          *reinterpret_cast<uint32_t*>(smem_raw + (q_addr - smem_u32(smem_raw)) + x * AT_BOX + off) =
+        for (int j = 0; j < OG; ++j) {
+          const uint32_t off = r * RB + ((j ^ swz) << 4) + 4 * quad;
+          *reinterpret_cast<uint32_t*>(smem_raw + (q_addr - smem_u32(smem_raw)) + x * BOX + off) =
               pack_h16x2(o[x][4 * j + 2 * hf] * inv, o[x][4 * j + 2 * hf + 1] * inv);
         }
       continue;
@@ -354,8 +375,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tm, const __grid_constant__
 #pragma unroll
     for (int x = 0; x < NB; ++x)
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint32_t*>(orow + 64 * x + 8 * j) =
+      for (int j = 0; j < OG; ++j)
+        *reinterpret_cast<uint32_t*>(orow + COLS * x + 8 * j) =
             pack_h16x2(o[x][4 * j + 2 * hf] * inv, o[x][4 * j + 2 * hf + 1] * inv);
   }
   if constexpr (EPI_ROLE) {

@@ -76,17 +76,19 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2-D half row-major [rows, cols] tensor, box = 64 columns (128 B, swizzle-128B) x box_rows.
+// 2-D half row-major [rows, cols] tensor, box = 64 columns (128 B, swizzle-128B) x box_rows, or with box_cols = 32
+// 32 columns (64 B, swizzle-64B: the head_dim-32 attention boxes).
 int make_tmap_h16(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols,
-                   uint32_t box_rows) {
+                   uint32_t box_rows, uint32_t box_cols = 64) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(B2E_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {cols * 2};
-  cuuint32_t box[2] = {64, box_rows};
+  cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(tm, B2E_TMAP_DTYPE, 2, const_cast<void*>(base), dims, strides,
-                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(B2E_ERR_CUDA, "cuTensorMapEncodeTiled(rows=%llu, cols=%llu, box_rows=%u) -> %d",
@@ -284,8 +286,8 @@ int launch_attention_kernel(const CUtensorMap& tm, const AttnScratch& sc, void* 
   auto kern = attention_kernel<D, MODE, V>;
   int rc = ensure_smem_attr(kern, Cfg::SMEM_BYTES);
   if (rc) return rc;
-  CUtensorMap tm_ctx = {};   // [B*S, heads*D], box 64 x 64: the epilogue role's TMA stores
-  if ((V & 128) && (rc = make_tmap_h16(&tm_ctx, ctx, (uint64_t)B * S, (uint64_t)heads * D, 64))) return rc;
+  CUtensorMap tm_ctx = {};   // [B*S, heads*D], box 64 x Cfg::COLS: the epilogue role's TMA stores
+  if ((V & 128) && (rc = make_tmap_h16(&tm_ctx, ctx, (uint64_t)B * S, (uint64_t)heads * D, 64, Cfg::COLS))) return rc;
   const float scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(D));
   const long long ctas = (long long)heads * B * ((S + Cfg::QT - 1) / Cfg::QT);
   if (ctas > 0x7fffffffLL)
@@ -355,29 +357,54 @@ int launch_attention_causal_d128(const void* qkv, AttnScratch& sc, void* ctx, in
   return launch_attention_kernel<128, 2, 0>(tm, sc, ctx, B, S, heads, kv_heads, window, st, lay);
 }
 
-#define DISPATCH_NV(H, CALL)                                        \
-  switch ((H) / 256) {                                              \
-    case 1: { constexpr int NV = 1; CALL; break; }                  \
-    case 2: { constexpr int NV = 2; CALL; break; }                  \
-    case 3: { constexpr int NV = 3; CALL; break; }                  \
-    case 4: { constexpr int NV = 4; CALL; break; }                  \
-    case 5: { constexpr int NV = 5; CALL; break; }                  \
-    case 8: { constexpr int NV = 8; CALL; break; }                  \
-    case 10: { constexpr int NV = 10; CALL; break; }                \
-    case 16: { constexpr int NV = 16; CALL; break; }                \
-    default: return fail(B2E_ERR_INVALID, "hidden size %d not supported (need 256*{1,2,3,4,5,8,10,16})", (H)); \
+// The one head_dim-32 instantiation (bidirectional, key-padding bias: MiniLM / BGE-small / E5-small, ESM-2 150M),
+// outside the variant switch: two consumer warpgroups, plain chunks from attn_prep, every thread storing its own
+// output pairs.  Measured on an H100 80GB HBM3 at a 700 W power limit, attn_prep + kernel, the eight combinations of
+// warpgroups x plain chunks x epilogue role side by side in one process (three runs each), bfloat16:
+//   MiniLM shape B=512 S=512, 12 heads, all rows full:  1.04-1.05 ms (variant 1) | 1.05-1.06 (129) | 1.09-1.10 (0,
+//                                                       193) | 1.26-1.32 (64, 192)
+//   the same, ragged lengths S/8..S:                    0.769-0.772 (1, 129) | 0.776 (128) | 0.78 (0) | 0.82 (193)
+//   ESM2-150M shape B=64 S=1026, 20 heads, ragged:      0.58-0.61 (0, 1, 128, 129) | 0.66-0.69 (193)
+// Four warpgroups lose here: with 32-column heads a chunk is too little work per CTA to pay for the wider CTA.
+constexpr int AT_D32_VARIANT = 1;
+
+// Bidirectional attention of the BERT and ESM-2 trunks by head_dim: the head_dim-64 kernel of the variant switch or
+// the head_dim-32 one.  tqkv: [T, 3H] with box 64 x head_dim (make_tmap_h16(..., AT_KC, head_dim)).
+int launch_attention_bidir(const CUtensorMap& tqkv, const AttnScratch& sc, void* ctx, int B, int S, int heads,
+                           int head_dim, cudaStream_t st, const SeqLayout& lay = SeqLayout()) {
+  if (head_dim == 32)
+    return launch_attention_kernel<32, 0, AT_D32_VARIANT>(tqkv, sc, ctx, B, S, heads, heads, 0, st, lay);
+  return launch_attention(tqkv, sc, ctx, B, S, heads, st, 0, lay);
+}
+
+// Row kernels are instantiated per hidden width HW (rowops.cuh: row_passes / row_lane_on); check_h accepts exactly
+// these widths.
+#define DISPATCH_H(H, CALL)                                         \
+  switch (H) {                                                      \
+    case 256: { constexpr int HW = 256; CALL; break; }              \
+    case 384: { constexpr int HW = 384; CALL; break; }              \
+    case 512: { constexpr int HW = 512; CALL; break; }              \
+    case 640: { constexpr int HW = 640; CALL; break; }              \
+    case 768: { constexpr int HW = 768; CALL; break; }              \
+    case 1024: { constexpr int HW = 1024; CALL; break; }            \
+    case 1280: { constexpr int HW = 1280; CALL; break; }            \
+    case 2048: { constexpr int HW = 2048; CALL; break; }            \
+    case 2560: { constexpr int HW = 2560; CALL; break; }            \
+    case 4096: { constexpr int HW = 4096; CALL; break; }            \
+    default: return fail(B2E_ERR_INVALID, "hidden size %d not supported (need 256*{1,2,3,4,5,8,10,16}, 384 or 640)", (H)); \
   }
 
 inline int row_blocks(int rows) { return (rows + ROW_WARPS - 1) / ROW_WARPS; }
 
-// The row kernels are instantiated per H/256 (DISPATCH_NV): reject every other width up front, i.e.
+// The row kernels are instantiated per width (DISPATCH_H): reject every other width up front, i.e.
 // at b2e_encoder_create, before any weight is touched, not at the first forward pass.
 int check_h(int H) {
-  if (H % 256 != 0) return fail(B2E_ERR_INVALID, "hidden size %d must be a multiple of 256", H);
+  if (H == 384 || H == 640) return B2E_OK;   // the two widths that end on a 128-column half pass
+  if (H % 256 != 0) return fail(B2E_ERR_INVALID, "hidden size %d must be a multiple of 256, or 384 or 640", H);
   switch (H / 256) {
     case 1: case 2: case 3: case 4: case 5: case 8: case 10: case 16: return B2E_OK;
   }
-  return fail(B2E_ERR_UNSUPPORTED, "hidden size %d not supported (built: 256 x {1,2,3,4,5,8,10,16})", H);
+  return fail(B2E_ERR_UNSUPPORTED, "hidden size %d not supported (built: 256 x {1,2,3,4,5,8,10,16}, 384, 640)", H);
 }
 
 // Pool-weight scratch shared by the fused and the standalone poolers.
@@ -677,14 +704,14 @@ int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate;
   int rc;
-  DISPATCH_NV(H, (embed_layernorm_kernel<NV><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (embed_layernorm_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      ids, types, e->word(), e->pos(), e->type(), e->emb_g(), e->emb_b(), e->hidden,
                      M, S, d.eps, lay.t_real, lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
 
   if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_kv64;
-  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT_KC))) return rc;
+  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv;
+  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, AT_KC, d.head_dim))) return rc;
   if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
@@ -693,13 +720,13 @@ int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
     if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, (const float*)e->L(l, 1), nullptr, M,
                           3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    if ((rc = launch_attention(tm_kv64, e->attn, e->ctx, B, S, d.heads, st, 0, lay)))
+    if ((rc = launch_attention_bidir(tm_qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
       return rc;
     // the residual add rides on the LayerNorm's coalesced reads, not on the GEMM epilogue
     if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, (const float*)e->L(l, 3), nullptr, M, H, H,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    DISPATCH_NV(H, (layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->tmp, e->hidden, (const float*)e->L(l, 4), (const float*)e->L(l, 5),
                        e->hidden, M, d.eps, lay.t_real)));
     if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, (const float*)e->L(l, 7), nullptr, M, I,
@@ -709,7 +736,7 @@ int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < d.num_layers) {
-      DISPATCH_NV(H, (layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->tmp, e->hidden, (const float*)e->L(l, 10), (const float*)e->L(l, 11),
                          e->hidden, M, d.eps, lay.t_real)));
     }
@@ -730,18 +757,18 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
   const int mask_token = d.reserved - 1;  // reserved = mask_token_id + 1, 0 = token dropout off
   int rc;
   esm_token_scale_kernel<<<(B + 7) / 8, 256, 0, st>>>(ids, mask, e->tok_scale, B, S, mask_token);
-  DISPATCH_NV(H, (esm_embed_kernel<NV><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (esm_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      ids, mask, (const float*)e->w[0], e->tok_scale, e->xres, M, S, mask_token, lay.t_real,
                      lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
   if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_kv64;
+  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv;
   if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT_KC))) return rc;
+  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, AT_KC, d.head_dim))) return rc;
 
-  DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      e->xres, nullptr, (const float*)e->E(0, 0), (const float*)e->E(0, 1), e->hidden,
                      M, d.eps, lay.t_real)));
   const long long rope_work = (long long)M * d.heads * 2;
@@ -749,14 +776,19 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
     if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, (const float*)e->E(l, 3), nullptr, M,
                           3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
-        e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
-    if ((rc = launch_attention(tm_kv64, e->attn, e->ctx, B, S, d.heads, st, 0, lay)))
+    if (d.head_dim == 32) {   // two threads per head of 2 x 16 frequencies
+      rope_halves_kernel<16><<<(unsigned)((rope_work * 2 + 255) / 256), 256, 0, st>>>(
+          e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
+    } else {
+      rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
+          e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
+    }
+    if ((rc = launch_attention_bidir(tm_qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
       return rc;
     if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, (const float*)e->E(l, 5), nullptr, M, H, H,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->E(l, 6), (const float*)e->E(l, 7), e->hidden,
                        M, d.eps, lay.t_real)));
     if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, (const float*)e->E(l, 9), nullptr, M, I, H,
@@ -766,7 +798,7 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
-      DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, (const float*)e->E(l + 1, 0), (const float*)e->E(l + 1, 1),
                          e->hidden, M, d.eps, lay.t_real)));
     }
@@ -785,7 +817,7 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   const int QC = e->qkv_cols(), CC = e->ctx_cols();
   int rc;
-  DISPATCH_NV(H, (mistral_embed_kernel<NV><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (mistral_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      ids, (const float*)e->w[0], e->xres, M, lay.t_real, lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
   if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
@@ -794,7 +826,7 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
   if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, CC, 128))) return rc;
   if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
 
-  DISPATCH_NV(H, (add_rmsnorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      e->xres, nullptr, (const float*)e->Mi(0, 0), e->hidden, M, d.eps, lay.t_real)));
   const int n_rot = d.heads + d.kv_heads;   // q heads and k heads are adjacent columns of qkv
   const long long rope_work = (long long)M * n_rot;
@@ -808,7 +840,7 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
       return rc;
     if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, CC, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    DISPATCH_NV(H, (add_rmsnorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->Mi(l, 3), e->hidden, M, d.eps, lay.t_real)));
     // gate and up in one GEMM (interleaved rows), silu(gate) * up in its epilogue: [M, I]
     if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H,
@@ -817,7 +849,7 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
     if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
-      DISPATCH_NV(H, (add_rmsnorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, (const float*)e->Mi(l + 1, 0), e->hidden, M, d.eps, lay.t_real)));
     }
   }
@@ -835,7 +867,7 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   int rc;
-  DISPATCH_NV(H, (modernbert_embed_kernel<NV><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (modernbert_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      ids, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2], e->xres,
                      e->hidden, M, d.eps, lay.t_real, lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
@@ -849,7 +881,7 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
   for (int l = 0; l < L; ++l) {
     const bool global = (l % d.global_every) == 0;
     if (l > 0) {
-      DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, (const float*)e->Mb(l, 0), (const float*)e->Mb(l, 1), e->hidden, M,
                          d.eps, lay.t_real)));
     }
@@ -863,7 +895,7 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
       return rc;
     if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->Mb(l, 4), (const float*)e->Mb(l, 5), e->hidden, M,
                        d.eps, lay.t_real)));
     // Wi with its input / gate halves interleaved: gelu(input) * gate in the epilogue -> [M, I]
@@ -948,6 +980,7 @@ int b2e_check_model(const B2EModelDesc* desc) {
     if (desc->sliding_window < 0) return fail(B2E_ERR_INVALID, "negative sliding_window");
     const int H = desc->hidden, I = desc->intermediate;
     const int QC = (desc->heads + 2 * desc->kv_heads) * 128, CC = desc->heads * 128;
+    if (H % 256 != 0) return fail(B2E_ERR_UNSUPPORTED, "Mistral: hidden size %d must be a multiple of 256", H);
     if ((rc = check_h(H))) return rc;
     if ((rc = check_gemm_shape(128, QC, H))) return rc;
     if ((rc = check_gemm_shape(128, H, CC))) return rc;
@@ -957,16 +990,21 @@ int b2e_check_model(const B2EModelDesc* desc) {
   if (desc->arch != B2E_ARCH_BERT && desc->arch != B2E_ARCH_ESM2 && desc->arch != B2E_ARCH_MODERNBERT)
     return fail(B2E_ERR_UNSUPPORTED, "arch %d: unknown architecture", desc->arch);
   if (desc->arch == B2E_ARCH_MODERNBERT) {
+    if (desc->head_dim != 64)
+      return fail(B2E_ERR_UNSUPPORTED, "ModernBERT: need head_dim 64 (got %d)", desc->head_dim);
+    if (desc->hidden % 256 != 0)
+      return fail(B2E_ERR_UNSUPPORTED, "ModernBERT: hidden size %d must be a multiple of 256", desc->hidden);
     if (desc->global_every <= 0) return fail(B2E_ERR_INVALID, "ModernBERT: global_every must be positive");
     if (desc->sliding_window <= 0) return fail(B2E_ERR_INVALID, "ModernBERT: sliding_window must be positive");
     if ((2 * desc->intermediate) % 256 != 0)
       return fail(B2E_ERR_UNSUPPORTED, "ModernBERT: 2 * intermediate_size = %d must be a multiple of 256 (the gated "
                   "epilogue pairs 128 input with 128 gate columns)", 2 * desc->intermediate);
   }
-  if (desc->head_dim != 64 || desc->heads * desc->head_dim != desc->hidden)
+  if ((desc->head_dim != 64 && desc->head_dim != 32) || desc->heads * desc->head_dim != desc->hidden)
     return fail(B2E_ERR_UNSUPPORTED,
-                "need head_dim 64 and heads*64 == hidden (got %d heads x %d, H=%d); of the ESM-2 family that "
-                "is esm2_t33_650M (H=1280) and esm2_t36_3B (H=2560)",
+                "need head_dim 64 or 32 and heads*head_dim == hidden (got %d heads x %d, H=%d); built: H in 256 x "
+                "{1,2,3,4,5,8,10,16}, 384 and 640 (MiniLM / BGE-small / E5-small: 384 = 12 x 32); of the ESM-2 family "
+                "that is esm2_t30_150M (H=640), esm2_t33_650M (H=1280) and esm2_t36_3B (H=2560)",
                 desc->heads, desc->head_dim, desc->hidden);
   if ((rc = check_h(desc->hidden))) return rc;
   if ((rc = check_gemm_shape(128, 3 * desc->hidden, desc->hidden))) return rc;
@@ -1089,7 +1127,11 @@ int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int
       b2e_encoder_destroy(e);
       return fail(B2E_ERR_CUDA, "cudaMalloc of the rotary tables failed");
     }
-    rope_table_kernel<<<(unsigned)((n + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos);
+    if (desc->head_dim == 32)   // [max_pos, 16]: angle(p, i) = p * 10000^(-2i/32)
+      rope_table_theta_kernel<<<(unsigned)((n / 2 + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos, 16,
+                                                                        10000.0f);
+    else
+      rope_table_kernel<<<(unsigned)((n + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos);
     if (cudaDeviceSynchronize() != cudaSuccess) {
       b2e_encoder_destroy(e);
       return fail(B2E_ERR_CUDA, "rotary table kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -1141,10 +1183,10 @@ int b2e_encode(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int
     if ((rc = run_mistral_trunk(e, ids, mask, B, S, st))) return rc;
     // final RMSNorm over (residual stream + last down_proj output)
     if (out_dtype == B2E_DTYPE_F32) {
-      DISPATCH_NV(H, (add_rmsnorm_kernel<NV, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_rmsnorm_kernel<HW, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, (const float*)e->w[1], (float*)out_hidden, M, d.eps)));
     } else {
-      DISPATCH_NV(H, (add_rmsnorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, (const float*)e->w[1], (h16*)out_hidden, M, d.eps)));
     }
     CUDA_TRY(cudaGetLastError());
@@ -1157,10 +1199,10 @@ int b2e_encode(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int
     const float* fg = (const float*)e->w[mb ? 3 : 1];
     const float* fb = (const float*)e->w[mb ? 4 : 2];
     if (out_dtype == B2E_DTYPE_F32) {
-      DISPATCH_NV(H, (add_layernorm_kernel<NV, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_layernorm_kernel<HW, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, fg, fb, (float*)out_hidden, M, d.eps)));
     } else {
-      DISPATCH_NV(H, (add_layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, fg, fb, (h16*)out_hidden, M, d.eps)));
     }
     CUDA_TRY(cudaGetLastError());
@@ -1168,11 +1210,11 @@ int b2e_encode(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int
   }
   if ((rc = run_bert_trunk(e, ids, mask, types, B, S, st))) return rc;
   if (out_dtype == B2E_DTYPE_F32) {
-    DISPATCH_NV(H, (layernorm_kernel<NV, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (layernorm_kernel<HW, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->tmp, e->hidden, (const float*)e->L(l, 10), (const float*)e->L(l, 11),
                        (float*)out_hidden, M, d.eps)));
   } else {
-    DISPATCH_NV(H, (layernorm_kernel<NV, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                        e->tmp, e->hidden, (const float*)e->L(l, 10), (const float*)e->L(l, 11),
                        (h16*)out_hidden, M, d.eps)));
   }
@@ -1202,7 +1244,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
       // only the B selected rows go through the final norm (fp32 end to end)
       seq_len_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, ps.seq_len, B, S);
       last_token_index_kernel<<<1, 256, 0, st>>>(mask, ps.seq_len, ps.idx, B, S);
-      DISPATCH_NV(H, (rmsnorm_gather_kernel<NV><<<row_blocks(B), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (rmsnorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, (const float*)e->w[1], ps.idx, out, B, S, d.eps, lay.cu)));
       if (l2) l2_normalize_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B, H);
       CUDA_TRY(cudaGetLastError());
@@ -1213,7 +1255,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
     const int nsplit = pool_nsplit(S);
     const int rows_per = (S + nsplit - 1) / nsplit;
     dim3 grid(B, nsplit);
-    DISPATCH_NV(H, (addnorm_pool_kernel<NV, true><<<grid, ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (addnorm_pool_kernel<HW, true><<<grid, ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, (const float*)e->w[1], nullptr, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
     CUDA_TRY(cudaGetLastError());
     return launch_finalize(ps, out, B, H, nsplit, l2, /*round_mode=*/0, st);
@@ -1228,7 +1270,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
       // only the B selected rows go through emb_layer_norm_after (fp32 end to end)
       seq_len_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, ps.seq_len, B, S);
       last_token_index_kernel<<<1, 256, 0, st>>>(mask, ps.seq_len, ps.idx, B, S);
-      DISPATCH_NV(H, (addnorm_gather_kernel<NV><<<row_blocks(B), ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (addnorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
                          e->xres, e->tmp, fg, fb, ps.idx, out, B, S, d.eps, lay.cu)));
       if (l2) l2_normalize_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B, H);
       CUDA_TRY(cudaGetLastError());
@@ -1239,7 +1281,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
     const int nsplit = pool_nsplit(S);
     const int rows_per = (S + nsplit - 1) / nsplit;
     dim3 grid(B, nsplit);
-    DISPATCH_NV(H, (addnorm_pool_kernel<NV, false><<<grid, ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (addnorm_pool_kernel<HW, false><<<grid, ROW_THREADS, 0, st>>>(
                        e->xres, e->tmp, fg, fb, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
     CUDA_TRY(cudaGetLastError());
     return launch_finalize(ps, out, B, H, nsplit, l2, /*round_mode=*/0, st);
@@ -1250,7 +1292,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
   if (pool_kind == B2E_POOL_LAST_TOKEN) {
     seq_len_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, ps.seq_len, B, S);
     last_token_index_kernel<<<1, 256, 0, st>>>(mask, ps.seq_len, ps.idx, B, S);
-    DISPATCH_NV(H, (layernorm_gather_kernel<NV><<<row_blocks(B), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (layernorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
                        e->tmp, e->hidden, ps.idx, g, bt, out, B, S, d.eps, lay.cu)));
     if (l2) l2_normalize_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B, H);
     CUDA_TRY(cudaGetLastError());
@@ -1262,7 +1304,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
   const int nsplit = pool_nsplit(S);
   const int rows_per = (S + nsplit - 1) / nsplit;
   dim3 grid(B, nsplit);
-  DISPATCH_NV(H, (layernorm_pool_kernel<NV><<<grid, ROW_THREADS, 0, st>>>(
+  DISPATCH_H(H, (layernorm_pool_kernel<HW><<<grid, ROW_THREADS, 0, st>>>(
                      e->tmp, e->hidden, g, bt, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
   CUDA_TRY(cudaGetLastError());
   return launch_finalize(ps, out, B, H, nsplit, l2, /*round_mode=*/0, st);
@@ -1381,17 +1423,17 @@ int b2e_pool_mean(const void* hidden, int dtype, int64_t* mask, int B, int S, in
   int round_mode = 0;
   switch (dtype) {
     case B2E_DTYPE_F32:
-      DISPATCH_NV(H, (pool_sum_kernel<NV, float><<<grid, ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (pool_sum_kernel<HW, float><<<grid, ROW_THREADS, 0, st>>>(
                          (const float*)hidden, ps.w, ps.part, S, rows_per)));
       break;
     case B2E_DTYPE_BF16:
       round_mode = 1;
-      DISPATCH_NV(H, (pool_sum_kernel<NV, bf16><<<grid, ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (pool_sum_kernel<HW, bf16><<<grid, ROW_THREADS, 0, st>>>(
                          (const bf16*)hidden, ps.w, ps.part, S, rows_per)));
       break;
     case B2E_DTYPE_F16:
       round_mode = 2;
-      DISPATCH_NV(H, (pool_sum_kernel<NV, __half><<<grid, ROW_THREADS, 0, st>>>(
+      DISPATCH_H(H, (pool_sum_kernel<HW, __half><<<grid, ROW_THREADS, 0, st>>>(
                          (const __half*)hidden, ps.w, ps.part, S, rows_per)));
       break;
     default:
@@ -1503,6 +1545,19 @@ int b2e_attention_d64(const void* qkv, const int64_t* mask, void* ctx, int B, in
   if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * 64, AT_KC))) return rc;
   if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
   return launch_attention(tkv, g_attn_scratch, ctx, B, S, heads, st);
+}
+
+int b2e_attention_d32(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads, void* stream) {
+  if (!qkv || !mask || !ctx) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (B <= 0 || S <= 0 || heads <= 0) return fail(B2E_ERR_INVALID, "empty attention problem");
+  int rc;
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  CUtensorMap tkv;
+  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * 32, AT_KC, 32))) return rc;
+  if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
+  return launch_attention_bidir(tkv, g_attn_scratch, ctx, B, S, heads, 32, st);
 }
 
 int b2e_attention_d64_window(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
@@ -1876,10 +1931,10 @@ int b2e_layernorm(const void* in, const float* gamma, const float* beta, void* o
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (out_dtype == B2E_DTYPE_F32) {
-    DISPATCH_NV(H, (layernorm_kernel<NV, float><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (layernorm_kernel<HW, float><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
                        (const h16*)in, nullptr, gamma, beta, (float*)out, rows, eps)));
   } else if (out_dtype == kStorageDtype) {
-    DISPATCH_NV(H, (layernorm_kernel<NV, h16><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
+    DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
                        (const h16*)in, nullptr, gamma, beta, (h16*)out, rows, eps)));
   } else {
     return fail(B2E_ERR_INVALID, "layernorm: out_dtype must be F32 or the storage type");

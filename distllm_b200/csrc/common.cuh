@@ -205,6 +205,18 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
   return d;
 }
 
+// The same with 64-byte swizzle (layout type 2): rows of 64 B, dense 8-row atoms 512 B apart (SBO = 512).  K-major:
+// a 64-byte row holds 32 h16 along K, two k16 steps (+2 in the address field each).  MN-major: one 64-byte row of
+// 32 M / N elements per K index, SBO steps 8 K rows; no caller is wider than 32 along M / N.
+__device__ __forceinline__ uint64_t make_smem_desc_sw64(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
+  d |= static_cast<uint64_t>(1u) << 16;
+  d |= static_cast<uint64_t>(512u >> 4) << 32;
+  d |= static_cast<uint64_t>(2) << 62;
+  return d;
+}
+
 #ifdef B2E_STORAGE_BF16
 #define B2E_WGMMA_AB "bf16.bf16"
 #else
@@ -237,6 +249,17 @@ __device__ __forceinline__ void wgmma_64x64_rs_tb(float (&d)[32], const uint32_t
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+
+// D[64 x 32] += A[64 x 16] (registers, as above) * B[16 x 32] (smem, MN-major)
+__device__ __forceinline__ void wgmma_64x32_rs_tb(float (&d)[16], const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.eq.u32 p, 1, 1;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32." B2E_WGMMA_AB " "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
 

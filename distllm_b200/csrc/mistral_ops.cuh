@@ -11,12 +11,12 @@ namespace b2e {
 
 // xres[row] = embed_tokens[ids[row]]   (fp32 residual stream; padding rows are embedded like any other
 // token, exactly as HF does -- they are only ever masked as KEYS)
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 mistral_embed_kernel(const int64_t* __restrict__ ids, const float* __restrict__ table,
                      float* __restrict__ xres, int rows, const int* __restrict__ n_dev = nullptr,
                      const int* __restrict__ tok_src = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -24,6 +24,7 @@ mistral_embed_kernel(const int64_t* __restrict__ ids, const float* __restrict__ 
   const int64_t id = ids[tok_src != nullptr ? __ldg(tok_src + row) : row];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) continue;
     const int c = v * 256 + lane * 8;
     float w[8];
     load8(table + static_cast<size_t>(id) * H + c, w);
@@ -31,10 +32,10 @@ mistral_embed_kernel(const int64_t* __restrict__ ids, const float* __restrict__ 
   }
 }
 
-template <int NV>
-__device__ __forceinline__ void warp_rmsnorm(float (&x)[NV][8], const float* __restrict__ gamma,
+template <int H>
+__device__ __forceinline__ void warp_rmsnorm(float (&x)[row_passes(H)][8], const float* __restrict__ gamma,
                                              int lane, float eps) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   float ss = 0.0f;
 #pragma unroll
   for (int v = 0; v < NV; ++v)
@@ -44,6 +45,7 @@ __device__ __forceinline__ void warp_rmsnorm(float (&x)[NV][8], const float* __r
   const float r = rsqrtf(ss * (1.0f / H) + eps);
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) continue;
     float g[8];
     load8(gamma + v * 256 + lane * 8, g);
 #pragma unroll
@@ -53,12 +55,12 @@ __device__ __forceinline__ void warp_rmsnorm(float (&x)[NV][8], const float* __r
 
 // Residual stream update fused with the next RMSNorm:
 //   xres += add (h16 GEMM output; nullptr on the very first call);  out = RMSNorm(xres) * gamma
-template <int NV, typename OutT>
+template <int H, typename OutT>
 __global__ void __launch_bounds__(ROW_THREADS)
 add_rmsnorm_kernel(float* __restrict__ xres, const h16* __restrict__ add,
                    const float* __restrict__ gamma, OutT* __restrict__ out, int rows, float eps,
                    const int* __restrict__ n_dev = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -66,6 +68,7 @@ add_rmsnorm_kernel(float* __restrict__ xres, const h16* __restrict__ add,
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const size_t off = static_cast<size_t>(row) * H + v * 256 + lane * 8;
     load8(xres + off, x[v]);
     if (add != nullptr) {
@@ -76,19 +79,20 @@ add_rmsnorm_kernel(float* __restrict__ xres, const h16* __restrict__ add,
       store8(xres + off, x[v]);
     }
   }
-  warp_rmsnorm<NV>(x, gamma, lane, eps);
+  warp_rmsnorm<H>(x, gamma, lane, eps);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + static_cast<size_t>(row) * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + static_cast<size_t>(row) * H + v * 256 + lane * 8, x[v]);
 }
 
 // Final norm for the last-token pooler: only the B selected rows are normalised.
 //   out[b] = RMSNorm(xres[b*S + idx[b]] + add[b*S + idx[b]]) * gamma        (fp32 [B,H])
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 rmsnorm_gather_kernel(const float* __restrict__ xres, const h16* __restrict__ add,
                       const float* __restrict__ gamma, const int* __restrict__ idx,
                       float* __restrict__ out, int B, int S, float eps, const int* __restrict__ cu = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (b >= B) return;
@@ -96,6 +100,7 @@ rmsnorm_gather_kernel(const float* __restrict__ xres, const h16* __restrict__ ad
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const size_t off = row * H + v * 256 + lane * 8;
     float a[8];
     load8(xres + off, x[v]);
@@ -103,19 +108,20 @@ rmsnorm_gather_kernel(const float* __restrict__ xres, const h16* __restrict__ ad
 #pragma unroll
     for (int e = 0; e < 8; ++e) x[v][e] += a[e];
   }
-  warp_rmsnorm<NV>(x, gamma, lane, eps);
+  warp_rmsnorm<H>(x, gamma, lane, eps);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + static_cast<size_t>(b) * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + static_cast<size_t>(b) * H + v * 256 + lane * 8, x[v]);
 }
 
 // ESM-2 last-token pooling: out[b] = LayerNorm(xres[row] + add[row]) for the B selected rows (fp32 [B,H]).
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 addnorm_gather_kernel(const float* __restrict__ xres, const h16* __restrict__ add,
                       const float* __restrict__ gamma, const float* __restrict__ beta,
                       const int* __restrict__ idx, float* __restrict__ out, int B, int S, float eps,
                       const int* __restrict__ cu = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (b >= B) return;
@@ -123,6 +129,7 @@ addnorm_gather_kernel(const float* __restrict__ xres, const h16* __restrict__ ad
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const size_t off = row * H + v * 256 + lane * 8;
     float a[8];
     load8(xres + off, x[v]);
@@ -130,22 +137,23 @@ addnorm_gather_kernel(const float* __restrict__ xres, const h16* __restrict__ ad
 #pragma unroll
     for (int e = 0; e < 8; ++e) x[v][e] += a[e];
   }
-  warp_layernorm<NV>(x, gamma, beta, lane, eps);
+  warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + static_cast<size_t>(b) * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + static_cast<size_t>(b) * H + v * 256 + lane * 8, x[v]);
 }
 
 // Final norm of the pre-norm families fused with the masked-sum pooling (the [B,S,H] final hidden state is
 // never written): x = xres + add, then LayerNorm (RMS == false: ESM-2's emb_layer_norm_after) or RMSNorm
 // (RMS == true: Mistral's final norm), weighted by the pooling weights and summed per block.
 // grid = (B, nsplit); each warp walks rows s = split*rows_per + warp, += ROW_WARPS (as layernorm_pool_kernel).
-template <int NV, bool RMS>
+template <int H, bool RMS>
 __global__ void __launch_bounds__(ROW_THREADS)
 addnorm_pool_kernel(const float* __restrict__ xres, const h16* __restrict__ add,
                     const float* __restrict__ gamma, const float* __restrict__ beta,
                     const float* __restrict__ w, float* __restrict__ part, int S, int rows_per, float eps,
                     const int* __restrict__ cu = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   __shared__ float red[H];
   const int b = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -162,6 +170,7 @@ addnorm_pool_kernel(const float* __restrict__ xres, const h16* __restrict__ add,
     const size_t row = (cu != nullptr ? static_cast<size_t>(__ldg(cu + b)) : static_cast<size_t>(b) * S) + s;
 #pragma unroll
     for (int v = 0; v < NV; ++v) {
+      if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
       const size_t off = row * H + v * 256 + lane * 8;
       float a[8];
       load8(xres + off, x[v]);
@@ -169,14 +178,14 @@ addnorm_pool_kernel(const float* __restrict__ xres, const h16* __restrict__ add,
 #pragma unroll
       for (int e = 0; e < 8; ++e) x[v][e] += a[e];
     }
-    if (RMS) warp_rmsnorm<NV>(x, gamma, lane, eps);
-    else warp_layernorm<NV>(x, gamma, beta, lane, eps);
+    if (RMS) warp_rmsnorm<H>(x, gamma, lane, eps);
+    else warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
     for (int v = 0; v < NV; ++v)
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[v][e] = fmaf(x[v][e], wv, acc[v][e]);
   }
-  block_store_partial<NV>(acc, red, part + (static_cast<size_t>(b) * nsplit + split) * H, warp, lane);
+  block_store_partial<H>(acc, red, part + (static_cast<size_t>(b) * nsplit + split) * H, warp, lane);
 }
 
 // cos/sin tables [max_pos, half]: angle(p, i) = p * theta^(-2i / (2*half))

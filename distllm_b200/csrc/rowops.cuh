@@ -13,6 +13,17 @@ namespace b2e {
 constexpr int ROW_WARPS = 8;
 constexpr int ROW_THREADS = ROW_WARPS * 32;
 
+// A row of H columns is held as row_passes(H) passes of 256 columns, lane owning columns v*256 + lane*8 .. +8 of
+// pass v.  The row kernels are instantiated per H (DISPATCH_H): 256 x {1,2,3,4,5,8,10,16}, 384 and 640.  A width with
+// a 128-column remainder ends on a half pass: there lanes 16-31 are off (row_lane_on), hold zeros, load and store
+// nothing and add nothing to the row statistics, which still divide by H.  For H % 256 == 0 the predicate is the
+// constant true and the kernels are the same code as with whole passes only.
+__host__ __device__ constexpr int row_passes(int H) { return (H + 255) / 256; }
+template <int H>
+__device__ __forceinline__ bool row_lane_on(int v, int lane) {
+  return H % 256 == 0 || v < H / 256 || lane < 16;
+}
+
 // ---- 8-element vector load/store helpers (lane owns columns v*256 + lane*8 .. +8)
 __device__ __forceinline__ void load8(const bf16* p, float (&v)[8]) {   // bf16 hidden states at the API
   const uint4 u = *reinterpret_cast<const uint4*>(p);
@@ -59,12 +70,18 @@ __device__ __forceinline__ void store8(float* p, const float (&v)[8]) {
   *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
   *reinterpret_cast<float4*>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
+__device__ __forceinline__ void zero8(float (&v)[8]) {   // the values of an off lane (row_lane_on)
+#pragma unroll
+  for (int e = 0; e < 8; ++e) v[e] = 0.0f;
+}
 
-// LayerNorm of one row held as NV x 8 values per lane (biased variance, like torch.layer_norm).
-template <int NV>
-__device__ __forceinline__ void warp_layernorm(float (&x)[NV][8], const float* __restrict__ gamma,
+// LayerNorm of one row held as NV x 8 values per lane (biased variance, like torch.layer_norm); the values of off
+// lanes (row_lane_on) are zeros.
+template <int H>
+__device__ __forceinline__ void warp_layernorm(float (&x)[row_passes(H)][8], const float* __restrict__ gamma,
                                                const float* __restrict__ beta, int lane, float eps) {
-  constexpr float inv_h = 1.0f / static_cast<float>(NV * 256);
+  constexpr int NV = row_passes(H);
+  constexpr float inv_h = 1.0f / static_cast<float>(H);
   float s = 0.0f;
 #pragma unroll
   for (int v = 0; v < NV; ++v)
@@ -73,15 +90,18 @@ __device__ __forceinline__ void warp_layernorm(float (&x)[NV][8], const float* _
   const float mean = warp_sum(s) * inv_h;
   float ss = 0.0f;
 #pragma unroll
-  for (int v = 0; v < NV; ++v)
+  for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) continue;
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       const float d = x[v][e] - mean;
       ss = fmaf(d, d, ss);
     }
+  }
   const float rstd = rsqrtf(warp_sum(ss) * inv_h + eps);
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) continue;
     float g[8], b[8];
     load8(gamma + v * 256 + lane * 8, g);
     load8(beta + v * 256 + lane * 8, b);
@@ -92,7 +112,7 @@ __device__ __forceinline__ void warp_layernorm(float (&x)[NV][8], const float* _
 
 // BERT embeddings: word[ids] + position[t % S] + type[type_ids] -> LayerNorm -> h16 hidden.
 // (transformers/models/bert/modeling_bert.py:72-112)
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 embed_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ type_ids,
                        const float* __restrict__ word, const float* __restrict__ pos,
@@ -100,7 +120,7 @@ embed_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restric
                        const float* __restrict__ beta, h16* __restrict__ out, int rows, int S,
                        float eps, const int* __restrict__ n_dev, const int* __restrict__ tok_src) {
   // n_dev / tok_src (nullable, pack.cuh): rows in use and the [B,S] position each packed row comes from
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -112,6 +132,7 @@ embed_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restric
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const int c = v * 256 + lane * 8;
     float w[8], q[8], t[8];
     load8(word + static_cast<size_t>(id) * H + c, w);
@@ -120,9 +141,10 @@ embed_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restric
 #pragma unroll
     for (int e = 0; e < 8; ++e) x[v][e] = (w[e] + t[e]) + q[e];  // HF order: (word + type) + pos
   }
-  warp_layernorm<NV>(x, gamma, beta, lane, eps);
+  warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + static_cast<size_t>(row) * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + static_cast<size_t>(row) * H + v * 256 + lane * 8, x[v]);
 }
 
 // x = in (+ resid when given): the residual add of the transformer block rides on the LayerNorm's
@@ -139,13 +161,13 @@ __device__ __forceinline__ void load8_residual(const h16* in, const h16* resid, 
 
 // LayerNorm over rows of a h16 matrix, optionally of (in + resid).  `out` may alias `resid`
 // (each warp reads its whole row before writing it).
-template <int NV, typename OutT>
+template <int H, typename OutT>
 __global__ void __launch_bounds__(ROW_THREADS)
 layernorm_kernel(const h16* __restrict__ in, const h16* resid, const float* __restrict__ gamma,
                  const float* __restrict__ beta, OutT* out, int rows, float eps,
                  const int* __restrict__ n_dev = nullptr, const int* __restrict__ out_row = nullptr) {
   // n_dev: device-resident row count; out_row: where each row goes in `out` (scatter back to [B,S])
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -153,23 +175,25 @@ layernorm_kernel(const h16* __restrict__ in, const h16* resid, const float* __re
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const size_t off = static_cast<size_t>(row) * H + v * 256 + lane * 8;
     load8_residual(in + off, resid ? resid + off : nullptr, x[v]);
   }
-  warp_layernorm<NV>(x, gamma, beta, lane, eps);
+  warp_layernorm<H>(x, gamma, beta, lane, eps);
   const size_t orow = out_row != nullptr ? static_cast<size_t>(__ldg(out_row + row)) : static_cast<size_t>(row);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + orow * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + orow * H + v * 256 + lane * 8, x[v]);
 }
 
 // LayerNorm of selected rows only: out[b] = LN(in[b*S + idx[b]])  (last-token pooling).
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 layernorm_gather_kernel(const h16* __restrict__ in, const h16* __restrict__ resid,
                         const int* __restrict__ idx, const float* __restrict__ gamma,
                         const float* __restrict__ beta, float* __restrict__ out, int B, int S,
                         float eps, const int* __restrict__ cu = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (b >= B) return;
@@ -177,12 +201,14 @@ layernorm_gather_kernel(const h16* __restrict__ in, const h16* __restrict__ resi
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const size_t off = row * H + v * 256 + lane * 8;
     load8_residual(in + off, resid ? resid + off : nullptr, x[v]);
   }
-  warp_layernorm<NV>(x, gamma, beta, lane, eps);
+  warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + static_cast<size_t>(b) * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + static_cast<size_t>(b) * H + v * 256 + lane * 8, x[v]);
 }
 
 // ------------------------------------------------------------------ pooling weights
@@ -261,20 +287,22 @@ __global__ void last_token_index_kernel(const int64_t* __restrict__ mask,
 
 // ------------------------------------------------------------------ masked-sum pooling
 // Shared tail: combine the ROW_WARPS per-warp partial column sums and write them to part[b,split,:].
-template <int NV>
-__device__ __forceinline__ void block_store_partial(float (&acc)[NV][8], float* red,
+template <int H>
+__device__ __forceinline__ void block_store_partial(float (&acc)[row_passes(H)][8], float* red,
                                                     float* __restrict__ part_row, int warp,
                                                     int lane) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   for (int w = 0; w < ROW_WARPS; ++w) {
     if (warp == w) {
 #pragma unroll
-      for (int v = 0; v < NV; ++v)
+      for (int v = 0; v < NV; ++v) {
+        if (!row_lane_on<H>(v, lane)) continue;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           const int c = v * 256 + lane * 8 + e;
           red[c] = (w == 0) ? acc[v][e] : red[c] + acc[v][e];
         }
+      }
     }
     __syncthreads();
   }
@@ -283,14 +311,14 @@ __device__ __forceinline__ void block_store_partial(float (&acc)[NV][8], float* 
 
 // Final-layer LayerNorm fused with masked-sum pooling: the [B,S,H] final hidden state is never
 // written.  grid = (B, nsplit); each warp walks rows s = split*rows_per + warp, += ROW_WARPS.
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 layernorm_pool_kernel(const h16* __restrict__ in, const h16* __restrict__ resid,
                       const float* __restrict__ gamma, const float* __restrict__ beta,
                       const float* __restrict__ w,
                       float* __restrict__ part, int S, int rows_per, float eps,
                       const int* __restrict__ cu = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   __shared__ float red[H];
   const int b = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -308,25 +336,26 @@ layernorm_pool_kernel(const h16* __restrict__ in, const h16* __restrict__ resid,
     const size_t row = (cu != nullptr ? static_cast<size_t>(__ldg(cu + b)) : static_cast<size_t>(b) * S) + s;
 #pragma unroll
     for (int v = 0; v < NV; ++v) {
+      if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
       const size_t off = row * H + v * 256 + lane * 8;
       load8_residual(in + off, resid ? resid + off : nullptr, x[v]);
     }
-    warp_layernorm<NV>(x, gamma, beta, lane, eps);
+    warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
     for (int v = 0; v < NV; ++v)
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[v][e] = fmaf(x[v][e], wv, acc[v][e]);
   }
-  block_store_partial<NV>(acc, red, part + (static_cast<size_t>(b) * nsplit + split) * H, warp,
+  block_store_partial<H>(acc, red, part + (static_cast<size_t>(b) * nsplit + split) * H, warp,
                           lane);
 }
 
 // Standalone masked-sum over a materialised hidden state (Pooler.pool API path).
-template <int NV, typename T>
+template <int H, typename T>
 __global__ void __launch_bounds__(ROW_THREADS)
 pool_sum_kernel(const T* __restrict__ in, const float* __restrict__ w, float* __restrict__ part,
                 int S, int rows_per) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   __shared__ float red[H];
   const int b = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -342,13 +371,14 @@ pool_sum_kernel(const T* __restrict__ in, const float* __restrict__ w, float* __
     const size_t row = static_cast<size_t>(b) * S + s;
 #pragma unroll
     for (int v = 0; v < NV; ++v) {
+      if (!row_lane_on<H>(v, lane)) continue;
       float x[8];
       load8(in + row * H + v * 256 + lane * 8, x);
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[v][e] = fmaf(x[e], wv, acc[v][e]);
     }
   }
-  block_store_partial<NV>(acc, red, part + (static_cast<size_t>(b) * nsplit + split) * H, warp,
+  block_store_partial<H>(acc, red, part + (static_cast<size_t>(b) * nsplit + split) * H, warp,
                           lane);
 }
 
@@ -478,13 +508,13 @@ __global__ void esm_token_scale_kernel(const int64_t* __restrict__ ids,
 
 // x[t,:] = word[ids[t]] (zero for <mask> tokens) * scale[b] * attention_mask[t]  -> fp32 residual stream
 // (modeling_esm.py:189-234 with rotary positions: no position table, no embedding LayerNorm)
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 esm_embed_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ mask,
                  const float* __restrict__ word, const float* __restrict__ scale,
                  float* __restrict__ xres, int rows, int S, int mask_token,
                  const int* __restrict__ n_dev = nullptr, const int* __restrict__ tok_src = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -495,6 +525,7 @@ esm_embed_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ ma
   if (mask_token >= 0 && id == mask_token) f = 0.0f;
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) continue;
     const int c = v * 256 + lane * 8;
     float w[8];
     load8(word + static_cast<size_t>(id) * H + c, w);
@@ -506,13 +537,13 @@ esm_embed_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ ma
 
 // ModernBERT embeddings (transformers/models/modernbert/modeling_modernbert.py:52-71): x = LayerNorm(tok[ids]);
 // x is the fp32 residual stream AND (layer 0 has no attn_norm: :318-320) the first attention input.
-template <int NV>
+template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 modernbert_embed_kernel(const int64_t* __restrict__ ids, const float* __restrict__ table,
                         const float* __restrict__ gamma, const float* __restrict__ beta,
                         float* __restrict__ xres, h16* __restrict__ hidden, int rows, float eps,
                         const int* __restrict__ n_dev = nullptr, const int* __restrict__ tok_src = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -520,10 +551,13 @@ modernbert_embed_kernel(const int64_t* __restrict__ ids, const float* __restrict
   const int64_t id = ids[tok_src != nullptr ? __ldg(tok_src + row) : row];
   float x[NV][8];
 #pragma unroll
-  for (int v = 0; v < NV; ++v) load8(table + static_cast<size_t>(id) * H + v * 256 + lane * 8, x[v]);
-  warp_layernorm<NV>(x, gamma, beta, lane, eps);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) load8(table + static_cast<size_t>(id) * H + v * 256 + lane * 8, x[v]);
+    else zero8(x[v]);
+  warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) continue;
     const size_t off = static_cast<size_t>(row) * H + v * 256 + lane * 8;
     store8(xres + off, x[v]);
     store8(hidden + off, x[v]);
@@ -533,12 +567,12 @@ modernbert_embed_kernel(const int64_t* __restrict__ ids, const float* __restrict
 // Residual stream update fused with the next LayerNorm (pre-LN blocks):
 //   xres += add (h16 GEMM output; nullptr on the very first call);  out = LayerNorm(xres)
 // The fp32 residual stream keeps 33 layers of accumulation out of h16.
-template <int NV, typename OutT>
+template <int H, typename OutT>
 __global__ void __launch_bounds__(ROW_THREADS)
 add_layernorm_kernel(float* __restrict__ xres, const h16* __restrict__ add,
                      const float* __restrict__ gamma, const float* __restrict__ beta,
                      OutT* __restrict__ out, int rows, float eps, const int* __restrict__ n_dev = nullptr) {
-  constexpr int H = NV * 256;
+  constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);
   if (n_dev != nullptr) rows = __ldg(n_dev);
@@ -546,6 +580,7 @@ add_layernorm_kernel(float* __restrict__ xres, const h16* __restrict__ add,
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
+    if (!row_lane_on<H>(v, lane)) { zero8(x[v]); continue; }
     const size_t off = static_cast<size_t>(row) * H + v * 256 + lane * 8;
     load8(xres + off, x[v]);
     if (add != nullptr) {
@@ -556,9 +591,10 @@ add_layernorm_kernel(float* __restrict__ xres, const h16* __restrict__ add,
       store8(xres + off, x[v]);
     }
   }
-  warp_layernorm<NV>(x, gamma, beta, lane, eps);
+  warp_layernorm<H>(x, gamma, beta, lane, eps);
 #pragma unroll
-  for (int v = 0; v < NV; ++v) store8(out + static_cast<size_t>(row) * H + v * 256 + lane * 8, x[v]);
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) store8(out + static_cast<size_t>(row) * H + v * 256 + lane * 8, x[v]);
 }
 
 // cos/sin tables for rotary embeddings, [max_pos, 32] each: angle(p, i) = p * 10000^(-2i/64)

@@ -49,7 +49,11 @@ class AutoEncoderConfig(BaseConfig):
 
 
 class AutoEncoder:
-    """Encoder for HF checkpoints of the BERT, ModernBERT and Mistral families on the native kernels."""
+    """Encoder for HF checkpoints of the BERT, ModernBERT and Mistral families on the native kernels.
+
+    Built shapes (``b2e_check_model``, checked before any weight is loaded): BERT with head_dim 64 or 32 and H in
+    256 x {1,2,3,4,5,8,10,16}, 384 or 640 (all-MiniLM-L6-v2, bge-small-en-v1.5, e5-small-v2: 384 = 12 x 32);
+    ModernBERT with head_dim 64 and Mistral with head_dim 128, both at H a multiple of 256."""
 
     def __init__(self, config: AutoEncoderConfig):
         from transformers import AutoConfig

@@ -23,7 +23,7 @@
  *   b2e_adjacent_cosine_dist distllm/embed/embedders/semantic_chunk.py:24-55
  *   b2e_topk_ip / b2e_topk_ip_tc / b2e_max_row_norm
  *                           distllm/rag/search.py:280-336 (exact float32 search of the query path)
- *   b2e_gemm_h16 / b2e_attention_d64 / b2e_attention_causal_d128 / b2e_layernorm: the building
+ *   b2e_gemm_h16 / b2e_attention_d64 / b2e_attention_d32 / b2e_attention_causal_d128 / b2e_layernorm: the building
  *                           blocks, exported so the parity tests can pin each kernel separately.
  */
 #ifndef B2E_H_
@@ -63,7 +63,7 @@ enum {
 typedef struct B2EModelDesc {
   int32_t arch;          /* B2E_ARCH_* */
   int32_t num_layers;
-  int32_t hidden;        /* H, multiple of 256 */
+  int32_t hidden;        /* H: see b2e_check_model */
   int32_t heads;
   int32_t kv_heads;
   int32_t head_dim;
@@ -93,7 +93,8 @@ int b2e_storage_dtype(void);
 const char* b2e_last_error(void);
 
 /* Number of device weight pointers b2e_encoder_create expects for `desc` (BERT: 5 + 12*L, ESM-2:
- * 3 + 12*L, Mistral: 2 + 6*L, ModernBERT: 5 + 8*L; order documented in distllm_b200/embed/encoders/weights.py).  Matrices
+ * 3 + 12*L, Mistral: 2 + 6*L, ModernBERT: 5 + 8*L, at every head_dim and width b2e_check_model accepts; order
+ * documented in distllm_b200/embed/encoders/weights.py).  Matrices
  * are of the build's 16-bit storage type (b2e_storage_dtype) [out,in] row-major, vectors and embedding
  * tables fp32.  Half values outside +-65504 saturate.  The pointers stay owned by the
  * caller and must outlive the handle.  For B2E_ARCH_ESM2, desc.reserved = mask_token_id + 1 enables
@@ -105,9 +106,10 @@ const char* b2e_last_error(void);
  * absent norm biases are passed as zero vectors, token_type_ids are ignored. */
 int b2e_num_weights(const B2EModelDesc* desc);
 /* Shape validation only (no device, no weights): 0 when b2e_encoder_create would accept `desc`,
- * else the error it would fail with.  BERT / ESM-2: head_dim 64, heads*64 == H, H in 256 x
- * {1,2,3,4,5,8,10,16}, I % 128 == 0; Mistral: head_dim 128 (see above).  Call it BEFORE uploading
- * weights (distllm/embed/encoders/auto.py:59-63 loads the checkpoint unconditionally). */
+ * else the error it would fail with.  BERT / ESM-2: head_dim 64 or 32, heads*head_dim == H, H in 256 x
+ * {1,2,3,4,5,8,10,16}, 384 or 640 (all-MiniLM-L6-v2, bge-small-en-v1.5, e5-small-v2: 384 = 12 x 32; esm2_t30_150M:
+ * 640 = 20 x 32), I % 128 == 0; Mistral: head_dim 128 (see above); Mistral and ModernBERT: H a multiple of 256.
+ * Call it BEFORE uploading weights (distllm/embed/encoders/auto.py:59-63 loads the checkpoint unconditionally). */
 int b2e_check_model(const B2EModelDesc* desc);
 int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int n_weights,
                        int device, B2EEncoder** out);
@@ -153,6 +155,9 @@ int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* re
 /* qkv [B*S, 3*heads*64] -> ctx [B*S, heads*64]; `reserved` must be NULL (it was a debug score dump). */
 int b2e_attention_d64(const void* qkv, const int64_t* attention_mask, void* ctx, int B, int S,
                       int heads, float* reserved, void* stream);
+/* The same at head_dim 32 (MiniLM / BGE-small / E5-small, ESM-2 150M): qkv [B*S, 3*heads*32] -> ctx [B*S, heads*32]. */
+int b2e_attention_d32(const void* qkv, const int64_t* attention_mask, void* ctx, int B, int S, int heads,
+                      void* stream);
 /* Same with a BIDIRECTIONAL sliding window: key j is visible to query i iff |i - j| <= window and
  * attention_mask[b,j] != 0 (window == 0: no window).  ModernBERT's local layers: HF
  * masking_utils.sliding_window_bidirectional_overlay with config.sliding_window = local_attention / 2. */
