@@ -21,8 +21,9 @@ STORAGE_TORCH_DTYPE = {'f16': torch.float16, 'bf16': torch.bfloat16}
 # inside the 1e-3 cosine tolerance against the fp32 reference; the 32-layer Mistral-7B shape needs half's three extra
 # significand bits (tools/drift_report.py measures the drift per layer; tests/test_gpu_config_parity.py holds every
 # family to the tolerance at configuration depth).  bench.py's extra.storage_ab times the same GEMM in both builds.
+# Qwen3 follows Mistral: Qwen3-Embedding-4B / 8B are 36 layers deep.
 # B2E_STORAGE=f16|bf16 overrides for every family.
-_STORAGE_BY_ARCH = {'bert': 'bf16', 'esm': 'bf16', 'modernbert': 'bf16', 'mistral': 'f16'}
+_STORAGE_BY_ARCH = {'bert': 'bf16', 'esm': 'bf16', 'modernbert': 'bf16', 'mistral': 'f16', 'qwen3': 'f16'}
 
 
 def storage_for_arch(arch: str) -> str:
@@ -43,7 +44,7 @@ def storage_of(dtype: torch.dtype) -> str:
             return name
     raise NativeError(f'no libb2e build stores {dtype}: expected float16 or bfloat16 operands')
 
-ARCH_BERT, ARCH_ESM2, ARCH_MISTRAL, ARCH_MODERNBERT = 0, 1, 2, 3
+ARCH_BERT, ARCH_ESM2, ARCH_MISTRAL, ARCH_MODERNBERT, ARCH_QWEN3 = 0, 1, 2, 3, 4
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2
 POOL_MEAN_REF, POOL_MEAN_PER_ROW, POOL_LAST_TOKEN = 0, 1, 2
 EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESID, EPI_SWIGLU, EPI_GEGLU = 0, 1, 2, 3, 4
@@ -72,6 +73,7 @@ EXPORTS = (
     'b2e_attention_d32',
     'b2e_attention_d64_window',
     'b2e_attention_causal_d128',
+    'b2e_qk_norm_rope',
     'b2e_topk_ip',
     'b2e_topk_ip_tc',
     'b2e_max_row_norm',
@@ -162,6 +164,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_attention_d64_window.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b2e_attention_causal_d128.restype = i32
     lib.b2e_attention_causal_d128.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    lib.b2e_qk_norm_rope.restype = i32
+    lib.b2e_qk_norm_rope.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, C.c_float, vp, vp, vp]
     lib.b2e_topk_ip.restype = i32
     lib.b2e_topk_ip.argtypes = [vp, i32, vp, i32, i64, i32, i32, vp, vp, vp]
     lib.b2e_topk_ip_tc.restype = i32
@@ -315,6 +319,31 @@ def attention_causal_d128(
         check(lib.b2e_attention_causal_d128(qkv.data_ptr(), attention_mask.data_ptr(), ctx.data_ptr(),
                                             batch, seq, heads, kv_heads, window, stream_ptr(qkv.device)), lib)
     return ctx
+
+
+def qk_norm_rope_(qkv: torch.Tensor, q_gamma: torch.Tensor, k_gamma: torch.Tensor, cos: torch.Tensor,
+                  sin: torch.Tensor, heads: int, kv_heads: int, eps: float, t_real: torch.Tensor | None = None,
+                  tok_src: torch.Tensor | None = None) -> torch.Tensor:
+    """Qwen3's q/k step in place on qkv [T, (heads + 2*kv_heads)*128] (q | k | v heads): per-head RMSNorm with
+    q_gamma / k_gamma (fp32 [128]), then rotary with cos / sin [S, 64] fp32 at position tok_src[t] % S (or t % S).
+    ``t_real``: int32 device tensor whose first element replaces T as the row count."""
+    lib = load(storage_of(qkv.dtype))
+    for t, what in ((qkv, 'qkv'), (q_gamma, 'q_gamma'), (k_gamma, 'k_gamma'), (cos, 'cos'), (sin, 'sin')):
+        _cuda_contig(t, what)
+    for t, what in ((t_real, 't_real'), (tok_src, 'tok_src')):
+        if t is not None and (_cuda_contig(t, what).dtype != torch.int32):
+            raise NativeError(f'{what} must be int32')
+    if q_gamma.dtype != torch.float32 or k_gamma.dtype != torch.float32 or cos.dtype != torch.float32 \
+            or sin.dtype != torch.float32:
+        raise NativeError('gains and rotary tables must be float32')
+    if qkv.shape[1] != (heads + 2 * kv_heads) * 128 or cos.shape[1] != 64 or q_gamma.numel() != 128 \
+            or k_gamma.numel() != 128:
+        raise NativeError('qk_norm_rope_: expected qkv [T, (heads + 2*kv_heads)*128], tables [S, 64], gains [128]')
+    with torch.cuda.device(qkv.device):
+        check(lib.b2e_qk_norm_rope(qkv.data_ptr(), q_gamma.data_ptr(), k_gamma.data_ptr(), cos.data_ptr(),
+                                   sin.data_ptr(), qkv.shape[0], cos.shape[0], heads, kv_heads, eps, _ptr(t_real),
+                                   _ptr(tok_src), stream_ptr(qkv.device)), lib)
+    return qkv
 
 
 def topk_ip(queries: torch.Tensor, corpus: torch.Tensor, k: int,

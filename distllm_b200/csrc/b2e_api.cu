@@ -514,6 +514,11 @@ thread_local AttnScratch g_attn_scratch;  // for the standalone attention op
 
 }  // namespace
 
+// The decoder family (Mistral, Qwen3): pre-RMSNorm blocks, head_dim-128 grouped-query causal attention, SwiGLU.
+// Qwen3 adds a per-head RMSNorm of q and k before the rotary embedding: two more weight slots per layer.
+inline bool is_decoder(int arch) { return arch == B2E_ARCH_MISTRAL || arch == B2E_ARCH_QWEN3; }
+inline int decoder_layer_slots(int arch) { return arch == B2E_ARCH_QWEN3 ? 8 : 6; }
+
 // ================================================================== encoder handle
 struct B2EEncoder {
   B2EModelDesc desc;
@@ -558,8 +563,8 @@ struct B2EEncoder {
 
   // Mistral family: fp32 residual stream and rotary tables as above; weight slots (weights.py):
   //   0 embed_tokens, 1 final norm; per layer (2 + 6 l): input norm, Wqkv, Wo, post-attention norm,
-  //   Wgu (gate/up interleaved), Wd
-  const void* Mi(int l, int k) const { return w[2 + 6 * l + k]; }
+  //   Wgu (gate/up interleaved), Wd; Qwen3 (2 + 8 l): the same six, then q_norm, k_norm (fp32 [128])
+  const void* Mi(int l, int k) const { return w[2 + decoder_layer_slots(desc.arch) * l + k]; }
   // ModernBERT: weight slots (weights.py): 0 tok_embeddings, 1/2 embeddings.norm g/b, 3/4 final_norm g/b; per
   // layer (5 + 8 l): attn_norm g/b, Wqkv, Wo, mlp_norm g/b, Wi (input/gate interleaved), mlp.Wo.  rope_cos/sin =
   // full-attention layers' table, rope_cos2/sin2 = sliding-attention layers'
@@ -581,19 +586,16 @@ struct B2EEncoder {
   }
 
   int qkv_cols() const {
-    return desc.arch == B2E_ARCH_MISTRAL ? (desc.heads + 2 * desc.kv_heads) * desc.head_dim
-                                         : 3 * desc.hidden;
+    return is_decoder(desc.arch) ? (desc.heads + 2 * desc.kv_heads) * desc.head_dim : 3 * desc.hidden;
   }
-  int ctx_cols() const {
-    return desc.arch == B2E_ARCH_MISTRAL ? desc.heads * desc.head_dim : desc.hidden;
-  }
+  int ctx_cols() const { return is_decoder(desc.arch) ? desc.heads * desc.head_dim : desc.hidden; }
   bool has_xres() const { return desc.arch != B2E_ARCH_BERT; }
 };
 
 namespace {
 
 size_t tokens_bytes(const B2EModelDesc& d, size_t tokens) {
-  if (d.arch == B2E_ARCH_MISTRAL)
+  if (is_decoder(d.arch))
     return tokens * (size_t)(2 * d.hidden + (2 * d.heads + 2 * d.kv_heads) * d.head_dim + d.intermediate) * 2;
   return tokens * (size_t)(6 * d.hidden + d.intermediate) * 2;
 }
@@ -811,6 +813,8 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
 // transformers/models/mistral/modeling_mistral.py:328-400 (model), :202-242 (block), :122-180
 // (attention), :35-48 (MLP).  Like the ESM-2 trunk it leaves xres (before the last MLP output is
 // added) and e->tmp (that down_proj output); the caller applies the final norm to xres + tmp.
+// Qwen3 (transformers/models/qwen3/modeling_qwen3.py) is the same block with q_norm / k_norm applied to every q
+// and k head before the rotary embedding: qk_rmsnorm_rope_kernel takes rope_halves_kernel<64>'s place.
 int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B, int S,
                       cudaStream_t st, const SeqLayout& lay = SeqLayout()) {
   const B2EModelDesc& d = e->desc;
@@ -833,8 +837,14 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
   for (int l = 0; l < L; ++l) {
     if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, QC, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    rope_halves_kernel<64><<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
-        e->qkv, e->rope_cos, e->rope_sin, M, S, n_rot, QC, lay.t_real, lay.tok_src);
+    if (d.arch == B2E_ARCH_QWEN3) {
+      qk_rmsnorm_rope_kernel<<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
+          e->qkv, (const float*)e->Mi(l, 6), (const float*)e->Mi(l, 7), e->rope_cos, e->rope_sin, M, S, d.heads,
+          d.kv_heads, QC, d.eps, lay.t_real, lay.tok_src);
+    } else {
+      rope_halves_kernel<64><<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
+          e->qkv, e->rope_cos, e->rope_sin, M, S, n_rot, QC, lay.t_real, lay.tok_src);
+    }
     if ((rc = launch_attention_causal_d128(e->qkv, e->attn, e->ctx, B, S, d.heads, d.kv_heads,
                                            d.sliding_window, st, lay)))
       return rc;
@@ -959,7 +969,7 @@ int b2e_num_weights(const B2EModelDesc* desc) {
   if (!desc) return -1;
   if (desc->arch == B2E_ARCH_BERT) return 5 + 12 * desc->num_layers;
   if (desc->arch == B2E_ARCH_ESM2) return 3 + 12 * desc->num_layers;
-  if (desc->arch == B2E_ARCH_MISTRAL) return 2 + 6 * desc->num_layers;
+  if (is_decoder(desc->arch)) return 2 + decoder_layer_slots(desc->arch) * desc->num_layers;
   if (desc->arch == B2E_ARCH_MODERNBERT) return 5 + 8 * desc->num_layers;
   return -1;
 }
@@ -971,16 +981,21 @@ int b2e_check_model(const B2EModelDesc* desc) {
   if (desc->num_layers <= 0 || desc->hidden <= 0 || desc->heads <= 0 || desc->intermediate <= 0)
     return fail(B2E_ERR_INVALID, "model description has a non-positive size");
   int rc;
-  if (desc->arch == B2E_ARCH_MISTRAL) {
+  if (is_decoder(desc->arch)) {
+    const char* fam = desc->arch == B2E_ARCH_QWEN3 ? "Qwen3" : "Mistral";
     if (desc->head_dim != 128 || desc->kv_heads <= 0 || desc->heads % desc->kv_heads != 0)
-      return fail(B2E_ERR_UNSUPPORTED, "need head_dim 128 and heads %% kv_heads == 0 (got %d/%d x %d)",
-                  desc->heads, desc->kv_heads, desc->head_dim);
+      return fail(B2E_ERR_UNSUPPORTED, "%s: need head_dim 128 and heads %% kv_heads == 0 (got %d/%d x %d)",
+                  fam, desc->heads, desc->kv_heads, desc->head_dim);
     if (desc->intermediate % 128 != 0)
-      return fail(B2E_ERR_UNSUPPORTED, "intermediate size %d must be a multiple of 128", desc->intermediate);
+      return fail(B2E_ERR_UNSUPPORTED, "%s: intermediate size %d must be a multiple of 128", fam,
+                  desc->intermediate);
     if (desc->sliding_window < 0) return fail(B2E_ERR_INVALID, "negative sliding_window");
+    if (desc->arch == B2E_ARCH_QWEN3 && desc->sliding_window != 0)
+      return fail(B2E_ERR_UNSUPPORTED, "Qwen3: sliding-window layers are not built (got sliding_window %d; built: "
+                  "full causal attention in every layer)", desc->sliding_window);
     const int H = desc->hidden, I = desc->intermediate;
     const int QC = (desc->heads + 2 * desc->kv_heads) * 128, CC = desc->heads * 128;
-    if (H % 256 != 0) return fail(B2E_ERR_UNSUPPORTED, "Mistral: hidden size %d must be a multiple of 256", H);
+    if (H % 256 != 0) return fail(B2E_ERR_UNSUPPORTED, "%s: hidden size %d must be a multiple of 256", fam, H);
     if ((rc = check_h(H))) return rc;
     if ((rc = check_gemm_shape(128, QC, H))) return rc;
     if ((rc = check_gemm_shape(128, H, CC))) return rc;
@@ -1013,7 +1028,7 @@ int b2e_check_model(const B2EModelDesc* desc) {
 }
 
 namespace {
-// Mistral family: head_dim 128, grouped-query heads, SwiGLU MLP, no biases.
+// Mistral family and Qwen3: head_dim 128, grouped-query heads, SwiGLU MLP, no biases.
 int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_weights, int device,
                    B2EEncoder** out) {
   const int L = desc->num_layers, H = desc->hidden, I = desc->intermediate;
@@ -1065,7 +1080,7 @@ int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int
                        int device, B2EEncoder** out) {
   if (!desc || !weights || !out) return fail(B2E_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (desc->arch == B2E_ARCH_MISTRAL) return create_mistral(desc, weights, n_weights, device, out);
+  if (is_decoder(desc->arch)) return create_mistral(desc, weights, n_weights, device, out);
   int rc;
   if ((rc = b2e_check_model(desc))) return rc;
   if (n_weights != b2e_num_weights(desc))
@@ -1179,7 +1194,7 @@ int b2e_encode(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int
   if ((rc = ensure_workspace(e, B, S))) return rc;
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, l = d.num_layers - 1;
-  if (d.arch == B2E_ARCH_MISTRAL) {
+  if (is_decoder(d.arch)) {
     if ((rc = run_mistral_trunk(e, ids, mask, B, S, st))) return rc;
     // final RMSNorm over (residual stream + last down_proj output)
     if (out_dtype == B2E_DTYPE_F32) {
@@ -1238,7 +1253,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
   // and attention query tiles; nothing here can observe a padded position.
   SeqLayout lay;
   if ((rc = pack_prepare(e, mask, B, S, packing_enabled(), st, &lay))) return rc;
-  if (d.arch == B2E_ARCH_MISTRAL) {
+  if (is_decoder(d.arch)) {
     if ((rc = run_mistral_trunk(e, ids, mask, B, S, st, lay))) return rc;
     if (pool_kind == B2E_POOL_LAST_TOKEN) {
       // only the B selected rows go through the final norm (fp32 end to end)
@@ -1572,6 +1587,24 @@ int b2e_attention_d64_window(const void* qkv, const int64_t* mask, void* ctx, in
   if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * 64, AT_KC))) return rc;
   if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
   return launch_attention(tkv, g_attn_scratch, ctx, B, S, heads, st, window);
+}
+
+int b2e_qk_norm_rope(void* qkv, const float* q_gamma, const float* k_gamma, const float* cos_t, const float* sin_t,
+                     int T, int S, int heads, int kv_heads, float eps, const int* t_real, const int* tok_src,
+                     void* stream) {
+  if (!qkv || !q_gamma || !k_gamma || !cos_t || !sin_t) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (T <= 0 || S <= 0 || heads <= 0 || kv_heads <= 0)
+    return fail(B2E_ERR_INVALID, "qk_norm_rope: bad problem T=%d S=%d heads=%d/%d", T, S, heads, kv_heads);
+  int rc;
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  const long long threads = (long long)T * (heads + kv_heads) * 8;
+  if ((threads + 255) / 256 > 0x7fffffffLL) return fail(B2E_ERR_INVALID, "qk_norm_rope: %lld threads", threads);
+  qk_rmsnorm_rope_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      static_cast<h16*>(qkv), q_gamma, k_gamma, cos_t, sin_t, T, S, heads, kv_heads, (heads + 2 * kv_heads) * 128,
+      eps, t_real, tok_src);
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
 }
 
 int b2e_attention_causal_d128(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,

@@ -201,4 +201,60 @@ __global__ void rope_table_theta_kernel(float* __restrict__ cos_t, float* __rest
   sin_t[i] = s;
 }
 
+// Qwen3 (transformers/models/qwen3/modeling_qwen3.py:248-249, :263-264): every q head and every k head of qkv
+// [T, ld] goes through its own RMSNorm over head_dim 128 BEFORE the rotary embedding, in place, one pass:
+//   y[i] = gamma[i] * (x[i] * rsqrt(mean(x^2) + eps)),   gamma = q_gamma for heads [0, heads), k_gamma for
+//   heads [heads, heads + kv_heads);  then the halves rotation of y at position tok_src[t] % S (or t % S).
+// Layout of rope_halves_kernel<64>: 8 threads per head, each owning frequencies [8g, 8g + 8) of both halves as
+// two 16-byte vectors; the head's sum of squares is reduced over its 8 lanes (8-aligned in the warp, since the
+// block size is a multiple of 8, and all 8 leave together past the last row).  One rounding to 16 bits, at the
+// store; the V heads behind the k heads are not touched.
+__global__ void __launch_bounds__(256)
+qk_rmsnorm_rope_kernel(h16* __restrict__ qkv, const float* __restrict__ q_gamma, const float* __restrict__ k_gamma,
+                       const float* __restrict__ cos_t, const float* __restrict__ sin_t, int T, int S, int heads,
+                       int kv_heads, int ld, float eps, const int* __restrict__ n_dev = nullptr,
+                       const int* __restrict__ tok_src = nullptr) {
+  constexpr int HALF = 64, TPH = HALF / 8;
+  if (n_dev != nullptr) T = __ldg(n_dev);
+  const int n_rot = heads + kv_heads;
+  const long long gtid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long unit = gtid / TPH;
+  const int g = static_cast<int>(gtid % TPH);
+  if (unit >= static_cast<long long>(T) * n_rot) return;
+  const int t = static_cast<int>(unit / n_rot);
+  const int hd = static_cast<int>(unit % n_rot);
+  h16* p = qkv + static_cast<size_t>(t) * ld + hd * (2 * HALF) + g * 8;
+  float x1[8], x2[8];
+  load8(p, x1);
+  load8(p + HALF, x2);
+  float ss = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) ss = fmaf(x2[i], x2[i], fmaf(x1[i], x1[i], ss));
+  const unsigned group = 0xffu << (threadIdx.x & 24);
+#pragma unroll
+  for (int o = TPH / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(group, ss, o);
+  const float r = rsqrtf(ss * (1.0f / (2 * HALF)) + eps);
+  const float* gamma = (hd < heads ? q_gamma : k_gamma) + g * 8;
+  float g1[8], g2[8];
+  load8(gamma, g1);
+  load8(gamma + HALF, g2);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    x1[i] = g1[i] * (x1[i] * r);
+    x2[i] = g2[i] * (x2[i] * r);
+  }
+  const int pos = (tok_src != nullptr ? __ldg(tok_src + t) : t) % S;
+  float c[8], sn[8];
+  load8(cos_t + static_cast<size_t>(pos) * HALF + g * 8, c);
+  load8(sin_t + static_cast<size_t>(pos) * HALF + g * 8, sn);
+  float o1[8], o2[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    o1[i] = x1[i] * c[i] - x2[i] * sn[i];
+    o2[i] = x2[i] * c[i] + x1[i] * sn[i];
+  }
+  store8(p, o1);
+  store8(p + HALF, o2);
+}
+
 }  // namespace b2e

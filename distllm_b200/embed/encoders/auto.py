@@ -19,14 +19,16 @@ from transformers import PreTrainedTokenizer
 from distllm_b200.embed.encoders.native import NativeBertEncoder
 from distllm_b200.embed.encoders.native import NativeMistralEncoder
 from distllm_b200.embed.encoders.native import NativeModernBertEncoder
+from distllm_b200.embed.encoders.native import NativeQwen3Encoder
 from distllm_b200.utils import BaseConfig
 
 # HF model_type -> native forward pass (BERT: post-LN encoder; Mistral: pre-RMSNorm decoder blocks
 # with rotary, grouped-query causal attention and SwiGLU, used as an encoder by the embedding models;
 # ModernBERT: pre-LN encoder with rotary, alternating full / sliding-window attention and GeGLU --
-# examples/embed/workstation/modernbert_semchunk.yaml:16-17)
+# examples/embed/workstation/modernbert_semchunk.yaml:16-17; Qwen3: the Mistral block with a per-head RMSNorm of q
+# and k before rotary -- Qwen3-Embedding 0.6B / 4B / 8B)
 _NATIVE_BY_MODEL_TYPE = {'bert': NativeBertEncoder, 'mistral': NativeMistralEncoder,
-                         'modernbert': NativeModernBertEncoder}
+                         'modernbert': NativeModernBertEncoder, 'qwen3': NativeQwen3Encoder}
 _SUPPORTED_MODEL_TYPES = tuple(_NATIVE_BY_MODEL_TYPE)
 
 
@@ -49,11 +51,13 @@ class AutoEncoderConfig(BaseConfig):
 
 
 class AutoEncoder:
-    """Encoder for HF checkpoints of the BERT, ModernBERT and Mistral families on the native kernels.
+    """Encoder for HF checkpoints of the BERT, ModernBERT, Mistral and Qwen3 families on the native kernels.
 
     Built shapes (``b2e_check_model``, checked before any weight is loaded): BERT with head_dim 64 or 32 and H in
     256 x {1,2,3,4,5,8,10,16}, 384 or 640 (all-MiniLM-L6-v2, bge-small-en-v1.5, e5-small-v2: 384 = 12 x 32);
-    ModernBERT with head_dim 64 and Mistral with head_dim 128, both at H a multiple of 256."""
+    ModernBERT with head_dim 64 at H a multiple of 256; Mistral and Qwen3 with head_dim 128 at a built H that is a
+    multiple of 256 (Qwen3-Embedding-0.6B / 4B / 8B: H = 1024 / 2560 / 4096), Qwen3 without sliding-window layers,
+    without attention biases and with default rotary."""
 
     def __init__(self, config: AutoEncoderConfig):
         from transformers import AutoConfig

@@ -163,6 +163,15 @@ class NativeMistralEncoder(NativeBertEncoder):
     _ARCH = 'mistral'
 
 
+class NativeQwen3Encoder(NativeBertEncoder):
+    """Qwen3 (Qwen3-Embedding): the Mistral-family trunk with a per-head RMSNorm of q and k before the rotary
+    embedding, fused with it in one kernel; ``token_type_ids`` unused."""
+
+    _DESC = staticmethod(W.qwen3_desc)
+    _WEIGHTS = staticmethod(W.qwen3_weight_list)
+    _ARCH = 'qwen3'
+
+
 class NativeModernBertEncoder(NativeBertEncoder):
     """ModernBERT (pre-LayerNorm blocks, rotary with one base per layer type, alternating full / sliding-window
     bidirectional attention, GeGLU) on the wgmma GEMMs and the head_dim-64 attention kernel with its

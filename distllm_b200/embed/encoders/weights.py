@@ -390,6 +390,70 @@ def random_mistral_state_dict(hf_config, seed: int = 0, device: torch.device | s
     return sd
 
 
+# ------------------------------------------------------------------------------ Qwen3
+# Qwen3 (``B2E_ARCH_QWEN3``), 2 + 8*L device tensors: Mistral's slots (HF ``Qwen3Model`` uses the same names), and
+# per layer two more:
+#       +6 self_attn.q_norm.weight [128] f32 (RMSNorm of every q head, before rotary)
+#       +7 self_attn.k_norm.weight [128] f32 (RMSNorm of every k head, before rotary)
+# Names are HF ``Qwen3Model`` state-dict keys (transformers/models/qwen3/modeling_qwen3.py).
+
+
+def qwen3_desc(hf_config) -> _native.ModelDesc:
+    """Translate a HF ``Qwen3Config`` into the C ``B2EModelDesc``; reject what is not built."""
+    if getattr(hf_config, 'attention_bias', False):
+        raise NotImplementedError('Qwen3: attention_bias=True is not built (built: q/k/v/o projections without '
+                                  'bias, as every Qwen3-Embedding checkpoint)')
+    types = list(getattr(hf_config, 'layer_types', None) or [])
+    if 'sliding_attention' in types:
+        raise NotImplementedError(f'Qwen3: sliding_attention layers (use_sliding_window) are not built (built: '
+                                  f'full causal attention in every layer; layer_types {types})')
+    params = getattr(hf_config, 'rope_parameters', None) or {}
+    if params.get('rope_type', 'default') != 'default':
+        raise NotImplementedError(f'Qwen3: rope_type {params["rope_type"]!r} is not built (built: default rotary)')
+    if getattr(hf_config, 'hidden_act', 'silu') != 'silu':
+        raise NotImplementedError(f'Qwen3: hidden_act={hf_config.hidden_act!r} is not built (built: SwiGLU, silu)')
+    desc = mistral_desc(hf_config)
+    desc.arch = _native.ARCH_QWEN3
+    desc.sliding_window = 0
+    return desc
+
+
+def qwen3_weight_list(
+    state_dict: Mapping[str, torch.Tensor],
+    num_layers: int,
+    device: torch.device,
+    dtype: torch.dtype = torch.float16,
+) -> list[torch.Tensor]:
+    """HF Qwen3Model (or ...ForCausalLM, ``model.`` prefix) state dict -> contiguous device tensors in ABI order."""
+    sd = {k[6:] if k.startswith('model.') else k: v for k, v in state_dict.items()}
+    mistral = mistral_weight_list(sd, num_layers, device, dtype)
+    out = mistral[:2]
+    for layer in range(num_layers):
+        p = f'layers.{layer}.self_attn.'
+        out += mistral[2 + 6 * layer:8 + 6 * layer]
+        out += [sd[p + n].detach().to(device=device, dtype=torch.float32).contiguous()
+                for n in ('q_norm.weight', 'k_norm.weight')]
+    return out
+
+
+def random_qwen3_state_dict(hf_config, seed: int = 0, device: torch.device | str = 'cpu',
+                            std: float | None = None,
+                            dtype: torch.dtype = torch.float32) -> dict[str, torch.Tensor]:
+    """Seeded random Qwen3 weights with HF Qwen3Model names (no ``model.`` prefix): Mistral's, then q_norm / k_norm
+    gains 1 + N(0, std) from a second generator (HF initialises them to ones, which would hide a missing or swapped
+    gain)."""
+    sd = random_mistral_state_dict(hf_config, seed=seed, device=device, std=std, dtype=dtype)
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed + 1)
+    std = getattr(hf_config, 'initializer_range', 0.02) if std is None else std
+    d = hf_config.head_dim
+    for layer in range(hf_config.num_hidden_layers):
+        for n in ('q_norm', 'k_norm'):
+            g = 1.0 + torch.randn(d, generator=gen, device=device, dtype=torch.float32) * std
+            sd[f'layers.{layer}.self_attn.{n}.weight'] = g.to(dtype)
+    return sd
+
+
 # ------------------------------------------------------------------------------ ModernBERT
 # ModernBERT (``B2E_ARCH_MODERNBERT``), 5 + 8*L device tensors (HF ``ModernBertModel`` names, ``model.`` prefix
 # stripped; transformers/models/modernbert/modeling_modernbert.py):

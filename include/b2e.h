@@ -11,7 +11,8 @@
  *   b2e_encode              distllm/embed/encoders/auto.py:119-138 (AutoEncoder.encode ->
  *                           HF BertModel.forward, transformers/models/bert/modeling_bert.py:628-690, or
  *                           HF MistralModel.forward, transformers/models/mistral/modeling_mistral.py:328-400, or
- *                           HF ModernBertModel.forward, transformers/models/modernbert/modeling_modernbert.py:424-490)
+ *                           HF ModernBertModel.forward, transformers/models/modernbert/modeling_modernbert.py:424-490, or
+ *                           HF Qwen3Model.forward, transformers/models/qwen3/modeling_qwen3.py)
  *                           and distllm/embed/encoders/esm2.py:109-134 (Esm2Encoder.encode -> HF
  *                           EsmForMaskedLM, transformers/models/esm/modeling_esm.py:189-516)
  *   b2e_encode_pooled       distllm/embed/embedders/full_sequence.py:59-69 (encode + pool + normalize)
@@ -23,8 +24,8 @@
  *   b2e_adjacent_cosine_dist distllm/embed/embedders/semantic_chunk.py:24-55
  *   b2e_topk_ip / b2e_topk_ip_tc / b2e_max_row_norm
  *                           distllm/rag/search.py:280-336 (exact float32 search of the query path)
- *   b2e_gemm_h16 / b2e_attention_d64 / b2e_attention_d32 / b2e_attention_causal_d128 / b2e_layernorm: the building
- *                           blocks, exported so the parity tests can pin each kernel separately.
+ *   b2e_gemm_h16 / b2e_attention_d64 / b2e_attention_d32 / b2e_attention_causal_d128 / b2e_qk_norm_rope /
+ *   b2e_layernorm:          the building blocks, exported so the parity tests can pin each kernel separately.
  */
 #ifndef B2E_H_
 #define B2E_H_
@@ -45,7 +46,7 @@ enum {
   B2E_ERR_NO_DEVICE = 4     /* no sm_90 device: there is no CPU fallback */
 };
 
-enum { B2E_ARCH_BERT = 0, B2E_ARCH_ESM2 = 1, B2E_ARCH_MISTRAL = 2, B2E_ARCH_MODERNBERT = 3 };
+enum { B2E_ARCH_BERT = 0, B2E_ARCH_ESM2 = 1, B2E_ARCH_MISTRAL = 2, B2E_ARCH_MODERNBERT = 3, B2E_ARCH_QWEN3 = 4 };
 enum { B2E_DTYPE_F32 = 0, B2E_DTYPE_BF16 = 1, B2E_DTYPE_F16 = 2 };
 enum {
   B2E_POOL_MEAN_REF = 0,     /* mean.py semantics incl. the cross-row end-token quirk (mean.py:36) */
@@ -93,7 +94,8 @@ int b2e_storage_dtype(void);
 const char* b2e_last_error(void);
 
 /* Number of device weight pointers b2e_encoder_create expects for `desc` (BERT: 5 + 12*L, ESM-2:
- * 3 + 12*L, Mistral: 2 + 6*L, ModernBERT: 5 + 8*L, at every head_dim and width b2e_check_model accepts; order
+ * 3 + 12*L, Mistral: 2 + 6*L, ModernBERT: 5 + 8*L, Qwen3: 2 + 8*L -- Mistral's six per layer, then q_norm and
+ * k_norm, fp32 [128] each, at every head_dim and width b2e_check_model accepts; order
  * documented in distllm_b200/embed/encoders/weights.py).  Matrices
  * are of the build's 16-bit storage type (b2e_storage_dtype) [out,in] row-major, vectors and embedding
  * tables fp32.  Half values outside +-65504 saturate.  The pointers stay owned by the
@@ -103,12 +105,15 @@ const char* b2e_last_error(void);
  * with rows interleaved in blocks of 64 (see B2E_EPI_SWIGLU), desc.sliding_window = 0 means none, and
  * token_type_ids are ignored.  For B2E_ARCH_MODERNBERT (head_dim 64, (2*intermediate) % 256 == 0, no Linear
  * biases) Wi is ONE matrix with its input / gate halves interleaved in blocks of 64 rows (B2E_EPI_GEGLU),
- * absent norm biases are passed as zero vectors, token_type_ids are ignored. */
+ * absent norm biases are passed as zero vectors, token_type_ids are ignored.  B2E_ARCH_QWEN3 is B2E_ARCH_MISTRAL
+ * with a per-head RMSNorm of every q and k head (over head_dim 128, epsilon desc.eps) before the rotary embedding;
+ * desc.sliding_window must be 0. */
 int b2e_num_weights(const B2EModelDesc* desc);
 /* Shape validation only (no device, no weights): 0 when b2e_encoder_create would accept `desc`,
  * else the error it would fail with.  BERT / ESM-2: head_dim 64 or 32, heads*head_dim == H, H in 256 x
  * {1,2,3,4,5,8,10,16}, 384 or 640 (all-MiniLM-L6-v2, bge-small-en-v1.5, e5-small-v2: 384 = 12 x 32; esm2_t30_150M:
- * 640 = 20 x 32), I % 128 == 0; Mistral: head_dim 128 (see above); Mistral and ModernBERT: H a multiple of 256.
+ * 640 = 20 x 32), I % 128 == 0; Mistral and Qwen3: head_dim 128 (see above); Mistral, Qwen3 and ModernBERT: H a
+ * multiple of 256 (heads*head_dim may differ from H for Mistral and Qwen3).
  * Call it BEFORE uploading weights (distllm/embed/encoders/auto.py:59-63 loads the checkpoint unconditionally). */
 int b2e_check_model(const B2EModelDesc* desc);
 int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int n_weights,
@@ -169,6 +174,13 @@ int b2e_attention_d64_window(const void* qkv, const int64_t* attention_mask, voi
  * and (window == 0 or i - j < window). */
 int b2e_attention_causal_d128(const void* qkv, const int64_t* attention_mask, void* ctx, int B, int S,
                               int heads, int kv_heads, int window, void* stream);
+/* Qwen3's q/k step, in place on qkv [T, (heads + 2*kv_heads)*128] (columns q heads | k heads | v heads): every q
+ * head x becomes rotary(q_gamma * x * rsqrt(mean(x^2) + eps)), every k head the same with k_gamma (fp32 [128]
+ * each); v heads are untouched.  cos_t / sin_t are [S, 64] fp32 (angle p * theta^(-2i/128)), the position of row t
+ * is tok_src[t] % S, or t % S when tok_src is NULL, and *t_real (device, nullable) replaces T as the row count. */
+int b2e_qk_norm_rope(void* qkv, const float* q_gamma, const float* k_gamma, const float* cos_t, const float* sin_t,
+                     int T, int S, int heads, int kv_heads, float eps, const int* t_real /* nullable */,
+                     const int* tok_src /* nullable */, void* stream);
 /* Exact inner-product top-k over a device-resident embedding matrix (the retrieval query path,
  * distllm/rag/search.py:280-336: faiss IndexFlatIP through semantic_search_faiss, float32/exact).
  * queries [Q,H] f32, corpus [N,H] F32 or BF16 (both row-major on the device), 1 <= k <= 256,

@@ -5,7 +5,7 @@ For each encoder family at its BASELINE shape, on N(0, 0.02) weights and on outl
 attended token's hidden state is compared with the oracle's state at the same depth: min / mean cosine per
 depth, plus the pooled embedding's cosine at full depth.  Writes a markdown table per case.
 
-usage: drift_report.py [out.md] [families: bert,esm,mistral]
+usage: drift_report.py [out.md] [families: bert,esm,mistral,qwen3]
 """
 import sys
 import time
@@ -27,7 +27,7 @@ def cos_rows(a, b):
 
 
 def set_layers(enc, n):
-    lib = nv.load()
+    lib = getattr(enc, '_lib', None) or nv.load()
     lib.b2e_debug_set_layers.argtypes = [type(enc._handle), __import__('ctypes').c_int]
     nv.check(lib.b2e_debug_set_layers(enc._handle, n))
 
@@ -143,6 +143,45 @@ def run_mistral(lines):
         torch.cuda.empty_cache()
 
 
+def run_qwen3(lines):
+    """Qwen3-Embedding-8B shape (36 layers, H 4096, 32 / 8 heads x 128, I 12288) in BOTH storage builds: the
+    measurement behind _native._STORAGE_BY_ARCH['qwen3']."""
+    from transformers import Qwen3Config
+
+    from distllm_b200.embed.encoders.native import NativeQwen3Encoder
+    from distllm_b200.embed.encoders.weights import random_qwen3_state_dict
+    from tools.oracle_qwen3 import qwen3_forward
+
+    cfg = Qwen3Config(vocab_size=32000, hidden_size=4096, num_hidden_layers=36, num_attention_heads=32,
+                      num_key_value_heads=8, head_dim=128, intermediate_size=12288, max_position_embeddings=32768,
+                      rms_norm_eps=1e-6, rope_parameters={'rope_type': 'default', 'rope_theta': 1e6},
+                      initializer_range=0.02, tie_word_embeddings=False)
+    dev = torch.device('cuda:0')
+    g = torch.Generator().manual_seed(24)
+    b, s = 2, 1024
+    ids = torch.randint(3, cfg.vocab_size, (b, s), generator=g)
+    lens = torch.tensor([1024, 700])
+    mask = (torch.arange(s)[None] < lens[:, None]).long()
+    for w in ('normal', 'outliers'):
+        sd = random_qwen3_state_dict(cfg, seed=6, device=dev, dtype=torch.float16)
+        if w == 'outliers':
+            add_outliers(sd, 'qwen3', seed=4)
+        t0 = time.time()
+        states = qwen3_forward(sd, cfg, ids, mask, return_all=True)
+        print(f'qwen3 oracle {time.time() - t0:.1f} s', flush=True)
+        ref_pool = opool.last_token_pool(states[-1], mask).numpy()
+        for storage in ('f16', 'bf16'):
+            enc = NativeQwen3Encoder(cfg, sd, storage=storage)
+            report(f'Qwen3-Embedding-8B shape, 36 layers, S=1024 (rows of 1024 and 700 tokens), {w} weights, '
+                   f'{storage} build (last_token pooler)', enc, ids, mask, None, states, ref_pool,
+                   nv.POOL_LAST_TOKEN, lines)
+            enc.close()
+            del enc
+            torch.cuda.empty_cache()
+        del sd, states
+        torch.cuda.empty_cache()
+
+
 if __name__ == '__main__':
     out = Path(sys.argv[1]) if len(sys.argv) > 1 else Path('gpurun_out/drift_report.md')
     fams = (sys.argv[2] if len(sys.argv) > 2 else 'bert,esm,mistral').split(',')
@@ -151,7 +190,7 @@ if __name__ == '__main__':
              'Model truncated to l layers on both sides (BERT: hidden_states[l]; ESM-2 / Mistral: final norm of the '
              'residual stream after l layers); cosine per attended token.  GEMMs multiply in bf16 with fp32 '
              'accumulation; norm statistics, softmax and pooling are fp32.']
-    for fam, fn in (('bert', run_bert), ('esm', run_esm), ('mistral', run_mistral)):
+    for fam, fn in (('bert', run_bert), ('esm', run_esm), ('mistral', run_mistral), ('qwen3', run_qwen3)):
         if fam in fams:
             fn(lines)
             out.parent.mkdir(parents=True, exist_ok=True)

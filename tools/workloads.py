@@ -101,6 +101,7 @@ _OUT_ROWS = {
     'bert': ('attention.output.dense.weight', 'output.dense.weight'),
     'esm': ('attention.output.dense.weight', 'output.dense.weight'),
     'mistral': ('self_attn.o_proj.weight', 'mlp.down_proj.weight'),
+    'qwen3': ('self_attn.o_proj.weight', 'mlp.down_proj.weight'),
     'modernbert': ('attn.Wo.weight', 'mlp.Wo.weight'),
 }
 
@@ -119,14 +120,21 @@ def add_outliers(state_dict: dict, family: str, seed: int = 0, n_massive: int = 
 
     (A first version drew EVERY gain from [0.1, 10]: with all q/k inputs up to 10x larger the attention
     logits grow ~100x, softmax turns into an arg-max, and the fp32 network itself becomes discontinuous in
-    its inputs -- any 16-bit implementation then flips keys at random tokens.)"""
+    its inputs -- any 16-bit implementation then flips keys at random tokens.)
+
+    Qwen3's per-head q_norm / k_norm gains ([head_dim], applied right before the attention logits) take no part
+    in the hidden-channel draws above; for the same reason they get log-uniform gains in ``gain_range`` only,
+    from a generator of their own, so the other families' weights are drawn exactly as before."""
     g = torch.Generator().manual_seed(seed)
     out_names = _OUT_ROWS[family]
     hidden = next(v.shape[0] for k, v in state_dict.items() if k.endswith(out_names[0]))
     perm = torch.randperm(hidden, generator=g)
     massive, loud = perm[:n_massive], perm[n_massive:n_massive + n_loud]
     lo, hi = float(np.log(gain_range[0])), float(np.log(gain_range[1]))
+    head_norms = ('self_attn.q_norm.weight', 'self_attn.k_norm.weight') if family == 'qwen3' else ()
     for name, t in state_dict.items():
+        if head_norms and name.endswith(head_norms):
+            continue
         if name.endswith(out_names):
             t[massive.to(t.device)] *= scale
         elif t.dim() == 1 and ('LayerNorm.weight' in name or 'layer_norm_after.weight' in name
@@ -138,4 +146,10 @@ def add_outliers(state_dict: dict, family: str, seed: int = 0, n_massive: int = 
             t.copy_(gain.to(device=t.device, dtype=t.dtype))
         elif t.dim() == 1 and ('LayerNorm.bias' in name or 'layer_norm_after.bias' in name):
             t.copy_((0.5 * torch.randn(t.shape, generator=g)).to(device=t.device, dtype=t.dtype))
+    if head_norms:
+        g_head = torch.Generator().manual_seed(seed + 1)
+        for name, t in state_dict.items():
+            if name.endswith(head_norms):
+                gain = torch.exp(torch.rand(t.shape, generator=g_head) * (hi - lo) + lo)
+                t.copy_(gain.to(device=t.device, dtype=t.dtype))
     return state_dict
