@@ -59,6 +59,7 @@ EXPORTS = (
     'b2e_num_weights',
     'b2e_check_model',
     'b2e_encoder_create',
+    'b2e_encoder_create_nf4',
     'b2e_encoder_destroy',
     'b2e_workspace_bytes',
     'b2e_encode',
@@ -69,6 +70,7 @@ EXPORTS = (
     'b2e_l2_normalize',
     'b2e_adjacent_cosine_dist',
     'b2e_gemm_h16',
+    'b2e_gemm_nf4',
     'b2e_attention_d64',
     'b2e_attention_d32',
     'b2e_attention_d64_window',
@@ -136,6 +138,9 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_check_model.argtypes = [C.POINTER(ModelDesc)]
     lib.b2e_encoder_create.restype = i32
     lib.b2e_encoder_create.argtypes = [C.POINTER(ModelDesc), C.POINTER(vp), i32, i32, C.POINTER(vp)]
+    lib.b2e_encoder_create_nf4.restype = i32
+    lib.b2e_encoder_create_nf4.argtypes = [C.POINTER(ModelDesc), C.POINTER(vp), i32, C.POINTER(vp), i32, i32,
+                                           C.POINTER(vp)]
     lib.b2e_encoder_destroy.restype = None
     lib.b2e_encoder_destroy.argtypes = [vp]
     lib.b2e_workspace_bytes.restype = i64
@@ -156,6 +161,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_adjacent_cosine_dist.argtypes = [vp, i32, i64, i32, vp, vp, vp]
     lib.b2e_gemm_h16.restype = i32
     lib.b2e_gemm_h16.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.b2e_gemm_nf4.restype = i32
+    lib.b2e_gemm_nf4.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b2e_attention_d64.restype = i32
     lib.b2e_attention_d64.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
     lib.b2e_attention_d32.restype = i32
@@ -258,6 +265,34 @@ def gemm_h16(
     out = torch.empty((m, n_out), dtype=a.dtype, device=a.device)
     with torch.cuda.device(a.device):
         check(lib.b2e_gemm_h16(a.data_ptr(), w.data_ptr(), _ptr(bias), _ptr(resid),
+                               out.data_ptr(), m, n, k, epilogue, stream_ptr(a.device)), lib)
+    return out
+
+
+def gemm_nf4(
+    a: torch.Tensor,
+    codes: torch.Tensor,
+    absmax: torch.Tensor,
+    bias: torch.Tensor | None,
+    resid: torch.Tensor | None = None,
+    epilogue: int = EPI_BIAS,
+) -> torch.Tensor:
+    """:func:`gemm_h16` with W in NF4 (embed/encoders/nf4.py: nf4_quantize): ``codes`` uint8 [N, K/2] and
+    ``absmax`` fp32 [K/64, N].  Equals bit for bit ``gemm_h16`` on the dequantised W in ``a``'s storage type."""
+    lib = load(storage_of(a.dtype))
+    _cuda_contig(a, 'a'), _cuda_contig(codes, 'codes'), _cuda_contig(absmax, 'absmax')
+    if bias is not None:
+        _cuda_contig(bias, 'bias')
+    m, k = a.shape
+    n = codes.shape[0]
+    if codes.dtype != torch.uint8 or absmax.dtype != torch.float32:
+        raise NativeError('gemm_nf4: codes must be uint8 and absmax float32')
+    if tuple(codes.shape) != (n, k // 2) or tuple(absmax.shape) != (k // 64, n):
+        raise NativeError(f'gemm_nf4: expected codes [{n}, {k // 2}] and absmax [{k // 64}, {n}] for K = {k}')
+    n_out = n // 2 if epilogue in (EPI_SWIGLU, EPI_GEGLU) else n
+    out = torch.empty((m, n_out), dtype=a.dtype, device=a.device)
+    with torch.cuda.device(a.device):
+        check(lib.b2e_gemm_nf4(a.data_ptr(), codes.data_ptr(), absmax.data_ptr(), _ptr(bias), _ptr(resid),
                                out.data_ptr(), m, n, k, epilogue, stream_ptr(a.device)), lib)
     return out
 

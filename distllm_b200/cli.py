@@ -36,7 +36,9 @@ def embed(  # noqa: PLR0913
     half_precision: bool = typer.Option(False, '--half_precision', '-hp', help='Return fp16 embeddings.'),
     eval_mode: bool = typer.Option(False, '--eval_mode', '-em', help='Set the model to evaluation mode.'),
     compile_model: bool = typer.Option(False, '--compile_model', '-cm', help='Accepted for compatibility.'),
-    quantization: bool = typer.Option(False, '--quantization', '-q', help='Accepted for compatibility.'),
+    quantization: bool = typer.Option(
+        False, '--quantization', '-q',
+        help='Hold the weight matrices in 4-bit NF4 on the GPU (bitsandbytes NF4 arithmetic, dequantised exactly).'),
 ) -> None:
     """Generate embeddings for every ``*.<data_extension>`` file under ``data_path``."""
     from distllm_b200.distributed_embedding import embedding_worker

@@ -96,6 +96,23 @@ int make_tmap_h16(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t col
   return B2E_OK;
 }
 
+// NF4 codes, uint8 row-major [rows, cols] (cols = K/2), box = 32 bytes (one k-block) x GEMM_BN rows, no swizzle
+int make_tmap_codes(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return fail(B2E_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {cols};
+  cuuint32_t box[2] = {GEMM_BK / 2, GEMM_BN};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(B2E_ERR_CUDA, "cuTensorMapEncodeTiled codes(rows=%llu, cols=%llu) -> %d", (unsigned long long)rows,
+                (unsigned long long)cols, (int)r);
+  return B2E_OK;
+}
+
 // 2-D float32 row-major tensor, box = 32 columns (128 bytes) x box_rows, 128-byte swizzle; rows beyond the
 // tensor read as zeros
 int make_tmap_f32(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
@@ -180,13 +197,30 @@ int check_gemm_shape(int M, int N, int K) {
 
 bool g_gemm_profiling = false;   // b2e_debug_set_clock_buffer: the bias GEMM runs its timeline instantiation
 
+// The W operand of a GEMM: a 16-bit [N,K] map (box 64 x GEMM_BN), or with absmax set the NF4 code map
+// (make_tmap_codes) and the block scales [K/64, N] it is dequantised with.
+struct GemmW {
+  CUtensorMap tm;
+  const float* absmax = nullptr;
+};
+
+int make_gemm_w(GemmW* w, const void* base, const float* absmax, uint64_t rows, uint64_t cols) {
+  w->absmax = absmax;
+  return absmax ? make_tmap_codes(&w->tm, base, rows, cols / 2) : make_tmap_h16(&w->tm, base, rows, cols, GEMM_BN);
+}
+
 template <int EPI>
-int launch_gemm_epi(const CUtensorMap& ta, const CUtensorMap& tb, void* out, const float* bias,
+int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const float* bias,
                     const h16* resid, int M, int N, int K, cudaStream_t st, const int* m_dev) {
   auto kern = gemm_h16_wgmma_kernel<EPI>;
-  if constexpr (EPI == EPI_BIAS)
+  int smem = GEMM_SMEM_BYTES;
+  if (wb.absmax) {
+    kern = gemm_h16_wgmma_kernel<EPI, false, true>;
+    smem = GemmPlan<true>::SMEM_BYTES;
+  } else if constexpr (EPI == EPI_BIAS) {
     if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true>;
-  int rc = ensure_smem_attr(kern, GEMM_SMEM_BYTES);
+  }
+  int rc = ensure_smem_attr(kern, smem);
   if (rc) return rc;
   DeviceInfo dev;
   if ((rc = current_device_info(&dev))) return rc;
@@ -196,15 +230,15 @@ int launch_gemm_epi(const CUtensorMap& ta, const CUtensorMap& tb, void* out, con
   if ((rc = make_tmap_h16(&tm_out, out, M, epi_is_glu(EPI) ? N / 2 : N, GEMM_BM))) return rc;
   // persistent: one CTA per SM (fewer for small problems), each walking its share of the tiles
   const unsigned grid = (unsigned)(tiles < dev.sms ? tiles : dev.sms);
-  kern<<<grid, GEMM_THREADS, GEMM_SMEM_BYTES, st>>>(ta, tb, tm_out, static_cast<h16*>(out), bias, resid, M, N, K,
-                                                    m_dev);
+  kern<<<grid, GEMM_THREADS, smem, st>>>(ta, wb.tm, tm_out, static_cast<h16*>(out), bias, resid, M, N, K, m_dev,
+                                         wb.absmax);
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
 }
 
-// A map: [M,K] box 128 rows; W map: [N,K] box GEMM_BN rows.
+// A map: [M,K] box 128 rows; W: see GemmW.
 // m_dev (nullable): device-resident row count <= M (packed token layout); M sizes the grid and the tensor maps.
-int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, void* out, const float* bias,
+int launch_gemm(const CUtensorMap& ta, const GemmW& tb, void* out, const float* bias,
                 const void* resid, int M, int N, int K, int epi, cudaStream_t st, const int* m_dev = nullptr) {
   const h16* r = static_cast<const h16*>(resid);
   switch (epi) {
@@ -535,8 +569,8 @@ struct B2EEncoder {
   int *pk_len_raw = nullptr, *pk_ok = nullptr, *pk_len = nullptr, *pk_cu = nullptr, *pk_treal = nullptr,
       *pk_src = nullptr;
   size_t pk_cap_b = 0, pk_cap_t = 0;
-  // weight tensor maps, one per layer
-  std::vector<CUtensorMap> tm_wqkv, tm_wo, tm_w1, tm_w2;
+  // weight operands, one per layer: 16-bit maps, or (b2e_encoder_create_nf4) code maps with their block scales
+  std::vector<GemmW> tm_wqkv, tm_wo, tm_w1, tm_w2;
   // host-loop staging
   int64_t* stage_in = nullptr;
   size_t stage_cap = 0;
@@ -1029,8 +1063,8 @@ int b2e_check_model(const B2EModelDesc* desc) {
 
 namespace {
 // Mistral family and Qwen3: head_dim 128, grouped-query heads, SwiGLU MLP, no biases.
-int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_weights, int device,
-                   B2EEncoder** out) {
+int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_weights, const float* const* absmax,
+                   int device, B2EEncoder** out) {
   const int L = desc->num_layers, H = desc->hidden, I = desc->intermediate;
   const int QC = (desc->heads + 2 * desc->kv_heads) * 128, CC = desc->heads * 128;
   int rc;
@@ -1051,10 +1085,11 @@ int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_w
   e->sms = info.sms;
   e->tm_wqkv.resize(L); e->tm_wo.resize(L); e->tm_w1.resize(L); e->tm_w2.resize(L);
   for (int l = 0; l < L; ++l) {
-    if ((rc = make_tmap_h16(&e->tm_wqkv[l], e->Mi(l, 1), QC, H, GEMM_BN)) ||
-        (rc = make_tmap_h16(&e->tm_wo[l], e->Mi(l, 2), H, CC, GEMM_BN)) ||
-        (rc = make_tmap_h16(&e->tm_w1[l], e->Mi(l, 4), 2 * I, H, GEMM_BN)) ||
-        (rc = make_tmap_h16(&e->tm_w2[l], e->Mi(l, 5), H, I, GEMM_BN))) {
+    const float* const* s = absmax ? absmax + 4 * l : nullptr;
+    if ((rc = make_gemm_w(&e->tm_wqkv[l], e->Mi(l, 1), s ? s[0] : nullptr, QC, H)) ||
+        (rc = make_gemm_w(&e->tm_wo[l], e->Mi(l, 2), s ? s[1] : nullptr, H, CC)) ||
+        (rc = make_gemm_w(&e->tm_w1[l], e->Mi(l, 4), s ? s[2] : nullptr, 2 * I, H)) ||
+        (rc = make_gemm_w(&e->tm_w2[l], e->Mi(l, 5), s ? s[3] : nullptr, H, I))) {
       delete e;
       return rc;
     }
@@ -1076,11 +1111,13 @@ int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_w
 }
 }  // namespace
 
-int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int n_weights,
-                       int device, B2EEncoder** out) {
+namespace {
+// absmax: nullptr (16-bit matrices) or 4 * num_layers NF4 scale pointers (b2e_encoder_create_nf4)
+int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_weights, const float* const* absmax,
+                   int device, B2EEncoder** out) {
   if (!desc || !weights || !out) return fail(B2E_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (is_decoder(desc->arch)) return create_mistral(desc, weights, n_weights, device, out);
+  if (is_decoder(desc->arch)) return create_mistral(desc, weights, n_weights, absmax, device, out);
   int rc;
   if ((rc = b2e_check_model(desc))) return rc;
   if (n_weights != b2e_num_weights(desc))
@@ -1109,10 +1146,11 @@ int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int
     const void* wo = mbert ? e->Mb(l, 3) : esm ? e->E(l, 4) : e->L(l, 2);
     const void* w1 = mbert ? e->Mb(l, 6) : esm ? e->E(l, 8) : e->L(l, 6);
     const void* w2 = mbert ? e->Mb(l, 7) : esm ? e->E(l, 10) : e->L(l, 8);
-    if ((rc = make_tmap_h16(&e->tm_wqkv[l], wqkv, 3 * H, H, GEMM_BN)) ||
-        (rc = make_tmap_h16(&e->tm_wo[l], wo, H, H, GEMM_BN)) ||
-        (rc = make_tmap_h16(&e->tm_w1[l], w1, n1, H, GEMM_BN)) ||
-        (rc = make_tmap_h16(&e->tm_w2[l], w2, H, I, GEMM_BN))) {
+    const float* const* s = absmax ? absmax + 4 * l : nullptr;
+    if ((rc = make_gemm_w(&e->tm_wqkv[l], wqkv, s ? s[0] : nullptr, 3 * H, H)) ||
+        (rc = make_gemm_w(&e->tm_wo[l], wo, s ? s[1] : nullptr, H, H)) ||
+        (rc = make_gemm_w(&e->tm_w1[l], w1, s ? s[2] : nullptr, n1, H)) ||
+        (rc = make_gemm_w(&e->tm_w2[l], w2, s ? s[3] : nullptr, H, I))) {
       delete e;
       return rc;
     }
@@ -1154,6 +1192,26 @@ int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int
   }
   *out = e;
   return B2E_OK;
+}
+}  // namespace
+
+int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int n_weights,
+                       int device, B2EEncoder** out) {
+  return create_encoder(desc, weights, n_weights, nullptr, device, out);
+}
+
+int b2e_encoder_create_nf4(const B2EModelDesc* desc, const void* const* weights, int n_weights,
+                           const float* const* absmax, int n_absmax, int device, B2EEncoder** out) {
+  if (!desc || !weights || !absmax || !out) return fail(B2E_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (n_absmax != 4 * desc->num_layers)
+    return fail(B2E_ERR_INVALID, "expected %d NF4 scale pointers (4 per layer), got %d", 4 * desc->num_layers,
+                n_absmax);
+  // the scales of a tile's k-block are one 512-byte bulk copy: 16-byte aligned
+  for (int i = 0; i < n_absmax; ++i)
+    if (!absmax[i] || reinterpret_cast<uintptr_t>(absmax[i]) % 16 != 0)
+      return fail(B2E_ERR_INVALID, "NF4 scale pointer %d is null or not 16-byte aligned", i);
+  return create_encoder(desc, weights, n_weights, absmax, device, out);
 }
 
 void b2e_encoder_destroy(B2EEncoder* e) {
@@ -1541,9 +1599,28 @@ int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* re
     return fail(B2E_ERR_INVALID, "gemm: the gated epilogues need N %% 256 == 0 (got %d)", N);
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
-  CUtensorMap ta, tb;
+  CUtensorMap ta;
+  GemmW tb;
   if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
-  if ((rc = make_tmap_h16(&tb, W, N, K, GEMM_BN))) return rc;
+  if ((rc = make_gemm_w(&tb, W, nullptr, N, K))) return rc;
+  return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
+}
+
+int b2e_gemm_nf4(const void* A, const void* codes, const float* absmax, const float* bias, const void* resid,
+                 void* out, int M, int N, int K, int epi, void* stream) {
+  if (!A || !codes || !absmax || !out) return fail(B2E_ERR_INVALID, "null tensor pointer");  // bias may be null
+  if (reinterpret_cast<uintptr_t>(absmax) % 16 != 0) return fail(B2E_ERR_INVALID, "absmax not 16-byte aligned");
+  if (epi == B2E_EPI_BIAS_RESID && !resid) return fail(B2E_ERR_INVALID, "resid epilogue needs resid");
+  int rc;
+  if ((rc = check_gemm_shape(M, N, K))) return rc;
+  if ((epi == B2E_EPI_SWIGLU || epi == B2E_EPI_GEGLU) && N % 256 != 0)
+    return fail(B2E_ERR_INVALID, "gemm: the gated epilogues need N %% 256 == 0 (got %d)", N);
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  CUtensorMap ta;
+  GemmW tb;
+  if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
+  if ((rc = make_gemm_w(&tb, codes, absmax, N, K))) return rc;
   return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
 }
 

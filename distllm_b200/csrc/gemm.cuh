@@ -13,6 +13,10 @@
 // each main loop, so the epilogue of one tile runs while the other consumer's main loop keeps the tensor cores
 // busy, and the two main loops never interleave.
 //
+// The NF4 instantiation (NF4 = true, quantization=True) differs only on the producer side: the W tile is written
+// into shared memory by the producer warpgroup from 4-bit codes and fp32 block scales (gemm_nf4_producer) instead of
+// being loaded by the TMA; consumers, hand-over, tile walk and epilogues are the same code.
+//
 // This replaces the cuBLAS nn.Linear calls HF BERT issues from
 // transformers/models/bert/modeling_bert.py:180-182 (q,k,v), :294-298 (attn out), :339-342 (FFN up +
 // GELU), :352-356 (FFN down), reached from distllm/embed/encoders/auto.py:135.
@@ -44,8 +48,46 @@ constexpr int GEMM_BAR_OFFSET = GEMM_OUT_OFFSET + 2 * 2 * GEMM_OUT_BOX;
 constexpr int GEMM_SMEM_BYTES = GEMM_BAR_OFFSET + 16 * GEMM_STAGES + 1024;   // + slack to align to 1024 B
 static_assert(GEMM_SMEM_BYTES <= 232448, "shared memory of one SM");
 // named barriers: GEMM_BAR_TURN + w = consumer w may issue its main loop; GEMM_BAR_STAGE + w = consumer w's
-// staging tile is free / written
-constexpr int GEMM_BAR_TURN = 1, GEMM_BAR_STAGE = 3;
+// staging tile is free / written; GEMM_BAR_NF4 = the NF4 producers have dequantised a k-block
+constexpr int GEMM_BAR_TURN = 1, GEMM_BAR_STAGE = 3, GEMM_BAR_NF4 = 5;
+
+// NF4 weights (embed/encoders/nf4.py: nf4_quantize): codes uint8 [N, K/2] (byte j of a row = column 2j in the
+// high nibble, 2j + 1 in the low one) and fp32 block scales absmax [K/64, N].  The producer warpgroup TMA-loads a
+// tile's 128 x 32-byte code box and its 128 scales (one contiguous 512-byte run) into a raw ring, and its 128
+// threads (one W row each) write round16(code[q] * absmax) into the stage's W region in the 128B-swizzled layout
+// the TMA gives a 16-bit W box: the wgmma sees byte for byte the tile of the 16-bit matrix dequantised on the host.
+// The raw ring costs a stage: four instead of five.
+constexpr int GEMM_NF4_RAW = 4;                                    // raw ring slots
+constexpr int GEMM_NF4_CODE_BYTES = GEMM_BN * GEMM_BK / 2;         // 128 rows x 32 bytes
+constexpr int GEMM_NF4_RAW_BYTES = GEMM_NF4_CODE_BYTES + GEMM_BN * 4;   // + 128 fp32 scales
+
+// Shared-memory plan and register split of one instantiation: [stages][output staging][raw ring][mbarriers]
+// [code table].  The 16-bit plan is the constants above.
+template <bool NF4>
+struct GemmPlan {
+  static constexpr int STAGES = NF4 ? 4 : GEMM_STAGES;
+  static constexpr int OUT_OFFSET = STAGES * GEMM_STAGE_BYTES;
+  static constexpr int RAW_OFFSET = OUT_OFFSET + 2 * 2 * GEMM_OUT_BOX;
+  static constexpr int BAR_OFFSET = RAW_OFFSET + (NF4 ? GEMM_NF4_RAW * GEMM_NF4_RAW_BYTES : 0);
+  // full[STAGES], empty[STAGES], then (NF4) raw_full[GEMM_NF4_RAW]
+  static constexpr int TABLE_OFFSET = BAR_OFFSET + 16 * STAGES + (NF4 ? 8 * GEMM_NF4_RAW : 0);
+  static constexpr int SMEM_BYTES = TABLE_OFFSET + (NF4 ? 16 * 4 : 0) + 1024;
+  // the dequantising producers need more than the TMA-only producer's 40 registers
+  static constexpr int PRODUCER_REGS = NF4 ? 56 : GEMM_PRODUCER_REGS;
+  static constexpr int CONSUMER_REGS = NF4 ? 224 : GEMM_CONSUMER_REGS;
+  // setmaxnreg moves registers within what the CTA was launched with (__launch_bounds__(384, 1): 168 per thread);
+  // a consumer's increase waits until the producers' decrease has freed enough, so a split beyond it never starts
+  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= GEMM_THREADS * 168, "registers the CTA holds");
+  static_assert(SMEM_BYTES <= 232448, "shared memory of one SM");
+};
+static_assert(GemmPlan<false>::SMEM_BYTES == GEMM_SMEM_BYTES && GemmPlan<false>::BAR_OFFSET == GEMM_BAR_OFFSET,
+              "the 16-bit plan");
+
+// bitsandbytes' NF4 code values (embed/encoders/nf4.py: NF4_CODE) as fp32 bit patterns
+__constant__ uint32_t kNf4CodeBits[16] = {
+    0xbf800000u, 0xbf3239b1u, 0xbf066b30u, 0xbeca32a0u, 0xbe91a24du, 0xbe3d353fu, 0xbdba7871u, 0x00000000u,
+    0x3da2faffu, 0x3e24cae3u, 0x3e7c04ddu, 0x3ead033au, 0x3ee1a4b8u, 0x3f1007abu, 0x3f3913b3u, 0x3f800000u,
+};
 
 // erf-GELU, x * Phi(x), with Phi from the Abramowitz-Stegun 7.1.26 erfc polynomial
 // (|erf error| <= 1.5e-7): gelu(x) = max(x,0) - 0.5*|x|*poly(t)*exp(-x^2/2), t = 1/(1 + p*|x|/sqrt2).
@@ -105,35 +147,141 @@ __device__ __forceinline__ GemmTiles gemm_tiles(int M, int N) {
   return {first, stride, first < tiles ? (tiles - 1 - first) / stride + 1 : 0, n_tiles};
 }
 
-template <int EPI, bool TL = false>
+// a read of data that stays constant once written (the NF4 code table): free to schedule, so that the producers
+// keep many lookups in flight
+__device__ __forceinline__ float ld_shared_const_f32(uint32_t addr) {
+  float v;
+  asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+
+// The NF4 producer warpgroup (all 128 threads; thread p dequantises W row p of every tile).  Thread 0 also issues
+// the loads: the A box of each k-block once its stage is free, and the code box + scales of the k-block
+// GEMM_NF4_RAW ahead into the raw slot the warpgroup has just finished reading.  A stage's full barrier completes
+// on the A bytes plus thread 0's arrival after the warpgroup's named-barrier sync.
+__device__ __forceinline__ void gemm_nf4_producer(const CUtensorMap* tm_a, const CUtensorMap* tm_codes,
+                                                  const float* __restrict__ absmax, const GemmTiles& tl, int N,
+                                                  int kblocks, uint32_t sb, uint32_t full_bar, uint32_t empty_bar) {
+  using P = GemmPlan<true>;
+  const int p = static_cast<int>(threadIdx.x) - 256;
+  const uint32_t raw0 = sb + P::RAW_OFFSET;
+  const uint32_t raw_bar = empty_bar + 8u * P::STAGES;
+  const uint32_t table = sb + P::TABLE_OFFSET;
+  const int total = tl.count * kblocks;
+  int ld = 0, ld_tile = 0, ld_kb = 0;   // thread 0: the next raw load (global k-block index, its tile and k-block)
+  auto load_raw = [&]() {
+    const int slot = ld % GEMM_NF4_RAW;
+    const int tile = tl.first + ld_tile * tl.stride;
+    const int n0 = (tile % tl.n_tiles) * GEMM_BN;
+    const uint32_t dst = raw0 + slot * GEMM_NF4_RAW_BYTES, bar = raw_bar + 8u * slot;
+    mbar_expect_tx(bar, GEMM_NF4_RAW_BYTES);
+    tma_load_2d(dst, tm_codes, bar, ld_kb * (GEMM_BK / 2), n0);
+    bulk_load_1d(dst + GEMM_NF4_CODE_BYTES, absmax + static_cast<size_t>(ld_kb) * N + n0, GEMM_BN * 4, bar);
+    ++ld;
+    if (++ld_kb == kblocks) { ld_kb = 0; ++ld_tile; }
+  };
+  if (p == 0) {
+    tma_prefetch_desc(tm_a);
+    tma_prefetch_desc(tm_codes);
+    while (ld < total && ld < GEMM_NF4_RAW) load_raw();
+  }
+  int stage = 0, slot = 0;
+  uint32_t phase = 0, raw_phase = 0;
+  for (int i = 0; i < tl.count; ++i) {
+    const int m0 = ((tl.first + i * tl.stride) / tl.n_tiles) * GEMM_BM;
+    for (int kb = 0; kb < kblocks; ++kb) {
+      mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
+      const uint32_t dst = sb + stage * GEMM_STAGE_BYTES;
+      const uint32_t fb = full_bar + 8u * stage;
+      if (p == 0) {
+        mbar_expect_tx(fb, GEMM_A_BYTES);
+        tma_load_2d(dst, tm_a, fb, kb * GEMM_BK, m0);
+      }
+      mbar_wait(raw_bar + 8u * slot, raw_phase);
+      const uint32_t src = raw0 + slot * GEMM_NF4_RAW_BYTES;
+      const uint4 c0 = ld_shared_v4(src + 32 * p), c1 = ld_shared_v4(src + 32 * p + 16);
+      const float s = ld_shared_f32(src + GEMM_NF4_CODE_BYTES + 4 * p);
+      const uint32_t words[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+      const uint32_t row = dst + GEMM_A_BYTES + 128 * p;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {   // 16-byte chunk c = columns [8c, 8c + 8) = code bytes [4c, 4c + 4)
+        uint32_t v[4];
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+          const uint32_t byte = (words[c] >> (8 * b)) & 0xffu;
+          // exactly nf4_dequantize's single fp32 product, then the storage rounding of weights.to_storage: bfloat16
+          // round-to-nearest-even, or (half) the +-65504 clamp and round-to-nearest, which cvt.rn.satfinite is
+          // for every finite product
+          const float lo = __fmul_rn(ld_shared_const_f32(table + ((byte >> 4) << 2)), s);
+          const float hi = __fmul_rn(ld_shared_const_f32(table + ((byte & 15u) << 2)), s);
+          v[b] = pack_h16x2(lo, hi);
+        }
+        st_shared_v4(row + ((c ^ (p & 7)) << 4), v[0], v[1], v[2], v[3]);
+      }
+      fence_proxy_async_smem();   // the W tile is read by wgmma (async proxy)
+      named_bar_sync(GEMM_BAR_NF4, 128);
+      if (p == 0) {
+        mbar_arrive(fb);
+        if (ld < total) load_raw();   // into the slot every producer has just read
+      }
+      if (++stage == P::STAGES) { stage = 0; phase ^= 1u; }
+      if (++slot == GEMM_NF4_RAW) { slot = 0; raw_phase ^= 1u; }
+    }
+  }
+}
+
+// NF4 = false: W is a 16-bit [N,K] map.  NF4 = true: tm_b is the uint8 code map [N,K/2] (box 32 x 128) and absmax
+// the block scales [K/64, N] (gemm_nf4_producer).
+template <int EPI, bool TL = false, bool NF4 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
                       const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x 128
                       const __grid_constant__ CUtensorMap tm_out,  // out [M,N] (GLU: [M,N/2]) box 64 x 128
                       h16* __restrict__ out, const float* __restrict__ bias, const h16* __restrict__ resid,
-                      int M, int N, int K, const int* __restrict__ m_dev) {
+                      int M, int N, int K, const int* __restrict__ m_dev, const float* __restrict__ absmax) {
+  using P = GemmPlan<NF4>;
   if (m_dev != nullptr) M = __ldg(m_dev);   // device-resident row count (packed token layout)
   const GemmTiles tl = gemm_tiles(M, N);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;   // the swizzled tiles need a 1024-byte aligned base
-  const uint32_t full_bar = sb + GEMM_BAR_OFFSET;
-  const uint32_t empty_bar = full_bar + 8u * GEMM_STAGES;
+  const uint32_t full_bar = sb + P::BAR_OFFSET;
+  const uint32_t empty_bar = full_bar + 8u * P::STAGES;
   const int warp = threadIdx.x >> 5;
   const int kblocks = K / GEMM_BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < GEMM_STAGES; ++s) {
-      mbar_init(full_bar + 8u * s, 1);
+    for (int s = 0; s < P::STAGES; ++s) {
+      mbar_init(full_bar + 8u * s, NF4 ? 2 : 1);   // NF4: the A bytes' expect_tx and the dequantisers' arrival
       mbar_init(empty_bar + 8u * s, 1);   // released by the one consumer whose tile the k-block belongs to
     }
+    if constexpr (NF4)
+      for (int s = 0; s < GEMM_NF4_RAW; ++s) mbar_init(empty_bar + 8u * (P::STAGES + s), 1);
     mbar_fence_init();
   }
+  if constexpr (NF4)
+    if (threadIdx.x < 16) st_shared_u32(sb + P::TABLE_OFFSET + 4 * threadIdx.x, kNf4CodeBits[threadIdx.x]);
   __syncthreads();
 
   long long* clk = (TL && blockIdx.x == 0) ? g_gemm_clock : nullptr;
   if (warp >= 8) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GEMM_PRODUCER_REGS));
-    if (warp == 8 && elect_one()) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(P::PRODUCER_REGS));
+    if constexpr (NF4) {
+      gemm_nf4_producer(&tm_a, &tm_b, absmax, tl, N, kblocks, sb, full_bar, empty_bar);
+    } else if (warp == 8 && elect_one()) {
       tma_prefetch_desc(&tm_a);
       tma_prefetch_desc(&tm_b);
       int stage = 0, n = 0;
@@ -156,12 +304,12 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
     return;
   }
 
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(GEMM_CONSUMER_REGS));
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(P::CONSUMER_REGS));
   const int wg = warp >> 2;
   const int t = threadIdx.x & 127;
   const int quad = t & 3;
   const int r_lo = 16 * (t >> 5) + ((t & 31) >> 2);   // row of acc[h][4j + {0,1}] in its 64-row half
-  const uint32_t stg = sb + GEMM_OUT_OFFSET + wg * (2 * GEMM_OUT_BOX);
+  const uint32_t stg = sb + P::OUT_OFFSET + wg * (2 * GEMM_OUT_BOX);
   int retired = 0;
   // Turn i (the CTA's i-th tile) belongs to consumer i % 2.  The hand-over into turn i (1 <= i < count) is one
   // arrive by the consumer of turn i - 1 after issuing its main loop and one sync by the consumer of turn i
@@ -175,8 +323,8 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
     if (i > 0) named_bar_sync(GEMM_BAR_TURN + wg, 256);
     // this tile's k-blocks follow the i * kblocks ones of the earlier turns in the ring
     const int it = i * kblocks;
-    int stage = it % GEMM_STAGES;
-    uint32_t phase = (it / GEMM_STAGES) & 1u;
+    int stage = it % P::STAGES;
+    uint32_t phase = (it / P::STAGES) & 1u;
     int prev = -1;
     for (int kb = 0; kb < kblocks; ++kb) {
       mbar_wait(full_bar + 8u * stage, phase);
@@ -202,7 +350,7 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
       if (TL && clk != nullptr && wg == 0 && t == 0 && retired < 256) clk[256 + retired] = clock64();
       ++retired;
       prev = stage;
-      if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
+      if (++stage == P::STAGES) { stage = 0; phase ^= 1u; }
     }
     if (i + 1 < tl.count) named_bar_arrive(GEMM_BAR_TURN + (wg ^ 1), 256);   // the other consumer's turn
     wgmma_wait<0>();

@@ -46,8 +46,12 @@ class AutoEncoderConfig(BaseConfig):
     eval_mode: bool = True
     # Kept for compatibility: there is no tracing compiler in this path
     compile_model: bool = False
-    # NF4 (bitsandbytes) weight quantisation, emulated at load time: the GEMMs run on dequant(quant(W))
+    # NF4 (bitsandbytes) weight quantisation: every transformer-block weight matrix is held on the device in 4-bit
+    # NF4 (3.56x less memory than 16 bits) and dequantised inside the GEMMs to exactly dequant(quant(W))
     quantization: bool = True
+    # With quantization: False dequantises once at load time into 16-bit matrices instead -- the same results bit for
+    # bit, 3.56x the weight memory, and the faster 16-bit GEMM (README: the NF4 GEMM runs at 0.64-0.78x of it)
+    nf4_storage: bool = True
 
 
 class AutoEncoder:
@@ -80,15 +84,24 @@ class AutoEncoder:
 
         self.config = config
         state_dict = model.state_dict()
+        nf4 = False
         if config.quantization:
             # the reference's default (auto.py:44-56): every nn.Linear weight goes through 4-bit NormalFloat with
             # double quantisation and is dequantised in front of each matmul -- what the GEMMs see is
-            # dequant(quant(W)).  That tensor is computed once here (embed/encoders/nf4.py restates bitsandbytes'
-            # published algorithm; the 4-bit STORAGE is not reproduced, the arithmetic is).
+            # dequant(quant(W)) (embed/encoders/nf4.py restates bitsandbytes' published algorithm).  The weights stay
+            # in NF4 on the device, quantised one matrix at a time, and the GEMMs dequantise them exactly.  A
+            # checkpoint whose quantised matrices are not all in 64-column blocks (no published checkpoint of a built
+            # family), or a config with nf4_storage: False, gets dequant(quant(W)) computed here once, in 16 bits: the
+            # same results, without the saving.
+            from distllm_b200.embed.encoders.nf4 import is_quantized_linear
+            from distllm_b200.embed.encoders.nf4 import nf4_storable
             from distllm_b200.embed.encoders.nf4 import quantize_state_dict_nf4
 
-            state_dict = quantize_state_dict_nf4(state_dict, device='cuda' if torch.cuda.is_available() else None)
-        self._native = _NATIVE_BY_MODEL_TYPE[hf_config.model_type](hf_config, state_dict)
+            nf4 = config.nf4_storage and all(nf4_storable(t) for name, t in state_dict.items()
+                                             if is_quantized_linear(name, t))
+            if not nf4:
+                state_dict = quantize_state_dict_nf4(state_dict, device='cuda' if torch.cuda.is_available() else None)
+        self._native = _NATIVE_BY_MODEL_TYPE[hf_config.model_type](hf_config, state_dict, nf4=nf4)
         del model, state_dict
         self._tokenizer = tokenizer
         self._dtype = torch.float16 if config.half_precision else torch.float32

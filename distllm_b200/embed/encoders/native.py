@@ -24,7 +24,12 @@ class NativeBertEncoder:
     _ARCH = 'bert'    # picks the build of the library (16-bit storage type): _native.storage_for_arch
 
     def __init__(self, hf_config, state_dict: Mapping[str, torch.Tensor],
-                 device: torch.device | str | None = None, storage: str | None = None) -> None:
+                 device: torch.device | str | None = None, storage: str | None = None, nf4: bool = False) -> None:
+        """``nf4``: hold every weight matrix in 4-bit NF4 (``b2e_encoder_create_nf4``), quantised from
+        ``state_dict`` one checkpoint matrix at a time on the device; the results equal bit for bit those of the
+        16-bit encoder built from ``nf4.quantize_state_dict_nf4(state_dict)``."""
+        if nf4 and self._ARCH == 'esm':
+            raise NotImplementedError('ESM-2 has no quantised configuration')
         self.storage = storage or _native.storage_for_arch(self._ARCH)
         lib = _native.load(self.storage)
         if not torch.cuda.is_available():
@@ -40,16 +45,23 @@ class NativeBertEncoder:
         _native.check(lib.b2e_check_model(C.byref(self.desc)), lib)
         self.hidden_size = hf_config.hidden_size
         self.max_positions = hf_config.max_position_embeddings
+        extra = {'matrix': W.nf4_matrix(self.device)} if nf4 else {}
         self._weights = self._WEIGHTS(state_dict, hf_config.num_hidden_layers, self.device,
-                                      _native.STORAGE_TORCH_DTYPE[self.storage])
+                                      _native.STORAGE_TORCH_DTYPE[self.storage], **extra)
+        self.nf4 = nf4
         n = len(self._weights)
         expected = lib.b2e_num_weights(C.byref(self.desc))
         if n != expected:
             raise _native.NativeError(f'weight list has {n} tensors, ABI expects {expected}')
-        ptrs = (C.c_void_p * n)(*[t.data_ptr() for t in self._weights])
+        ptrs = (C.c_void_p * n)(*[(t.codes if isinstance(t, W.Nf4Matrix) else t).data_ptr() for t in self._weights])
         handle = C.c_void_p()
-        _native.check(lib.b2e_encoder_create(C.byref(self.desc), ptrs, n, self.device.index,
-                                             C.byref(handle)), lib)
+        if nf4:
+            scales = [t.absmax.data_ptr() for t in self._weights if isinstance(t, W.Nf4Matrix)]
+            _native.check(lib.b2e_encoder_create_nf4(C.byref(self.desc), ptrs, n, (C.c_void_p * len(scales))(*scales),
+                                                     len(scales), self.device.index, C.byref(handle)), lib)
+        else:
+            _native.check(lib.b2e_encoder_create(C.byref(self.desc), ptrs, n, self.device.index,
+                                                 C.byref(handle)), lib)
         self._handle = handle
         self._lib = lib
 
@@ -86,6 +98,10 @@ class NativeBertEncoder:
         if t.dim() != 2:
             raise _native.NativeError(f'{name} must be [B,S]')
         return t
+
+    def weight_bytes(self) -> dict[str, int]:
+        """Device bytes of the weights: ``matrix`` (16-bit matrices, or NF4 codes + scales) and ``other``."""
+        return W.device_weight_bytes(self._weights)
 
     def workspace_bytes(self, batch: int, seq: int) -> int:
         return int(self._lib.b2e_workspace_bytes(self._handle, batch, seq))

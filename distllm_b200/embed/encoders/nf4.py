@@ -4,8 +4,18 @@ distllm/embed/encoders/auto.py:44-56 loads the checkpoint with
 ``BitsAndBytesConfig(load_in_4bit=True, bnb_4bit_quant_type='nf4', bnb_4bit_use_double_quant=True,
 bnb_4bit_compute_dtype=torch.bfloat16)``: every ``nn.Linear`` weight of the model is stored as 4-bit NormalFloat
 codes and DEQUANTISED to the compute dtype in front of each matmul.  What reaches the GEMMs is therefore
-``dequant(quant(W))``; this module computes exactly that tensor once, at load time, and hands it to the native
-16-bit GEMMs (the 4-bit storage itself -- a memory saving, not an arithmetic one -- is not reproduced).
+``dequant(quant(W))``.  This module quantises once, at load time, into the device format of the native NF4 GEMM
+(:func:`nf4_quantize`): per ``[N, K]`` matrix (``K % 64 == 0``, so that every 64-element block is one (row, k-block))
+
+  codes   uint8 [N, K/2], row-major; byte j of a row holds column 2j in its high nibble and 2j+1 in its low nibble
+  absmax  fp32 [K/64, N], k-block major: the double-quantised block scale absmax' (the fp32 value the dequantisation
+          multiplies by, not its 8-bit code), so one tile's 128 scales of a k-block are one 512-byte run
+
+and the GEMM computes ``round16(code[q] * absmax')`` in front of the tensor cores: the same single fp32 product as
+:func:`nf4_dequantize`, rounded as ``weights.to_storage`` rounds, i.e. bit for bit the 16-bit matrix
+``to_storage(nf4_roundtrip(W))``.  That costs 0.5625 bytes per weight (3.56x less than 16 bits); bitsandbytes'
+own storage is ~0.516 bytes, because it keeps the scales as 8-bit codes -- storing the reconstructed fp32 scale is
+what makes the GEMM's arithmetic exactly the load-time round trip's.
 
 bitsandbytes (pin >=0.42.0, pyproject.toml) is absent from this image and cannot run on CPU, so this restates
 its published algorithm -- PARITY UNPINNED for this branch:
@@ -50,22 +60,24 @@ def _nearest(values: torch.Tensor, code: torch.Tensor) -> torch.Tensor:
     return torch.bucketize(values, mid.to(values.device))
 
 
+BLOCK = 64
+_CHUNK_BLOCKS = 1 << 16   # blocks per step of the code search: bounds its temporaries to ~50 MB
+
+
 @torch.no_grad()
-def nf4_roundtrip(weight: torch.Tensor, blocksize: int = 64, double_quant: bool = True) -> torch.Tensor:
-    """``dequantize_4bit(quantize_4bit(weight))`` as fp32, same shape and device as ``weight``."""
-    w = weight.detach().to(torch.float32)
-    flat = w.flatten()
-    n = flat.numel()
-    pad = (-n) % blocksize
-    if pad:
-        flat = torch.cat([flat, flat.new_zeros(pad)])
-    blocks = flat.view(-1, blocksize)
-    absmax = blocks.abs().amax(dim=1)
-    code = torch.tensor(NF4_CODE, dtype=torch.float32, device=w.device)
+def _quantize_blocks(blocks: torch.Tensor, double_quant: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """fp32 ``[n_blocks, blocksize]`` -> (codes uint8 ``[n_blocks, blocksize/2]`` packed two per byte, high nibble first; absmax'
+    fp32 ``[n_blocks]``).  The code search runs in chunks of blocks so that no full-size temporary is made."""
+    code = torch.tensor(NF4_CODE, dtype=torch.float32, device=blocks.device)
+    absmax = torch.cat([blocks[i:i + _CHUNK_BLOCKS].abs().amax(dim=1)
+                        for i in range(0, blocks.shape[0], _CHUNK_BLOCKS)])
     safe = torch.where(absmax > 0, absmax, torch.ones_like(absmax))
-    q4 = _nearest(blocks / safe[:, None], code)
+    codes = torch.empty((blocks.shape[0], blocks.shape[1] // 2), dtype=torch.uint8, device=blocks.device)
+    for i in range(0, blocks.shape[0], _CHUNK_BLOCKS):
+        q4 = _nearest(blocks[i:i + _CHUNK_BLOCKS] / safe[i:i + _CHUNK_BLOCKS, None], code).to(torch.uint8)
+        codes[i:i + _CHUNK_BLOCKS] = (q4[:, 0::2] << 4) | q4[:, 1::2]
     if double_quant:
-        code8 = dynamic_map_8bit().to(w.device)
+        code8 = dynamic_map_8bit().to(blocks.device)
         offset = absmax.mean()
         centred = absmax - offset
         pad2 = (-centred.numel()) % 256
@@ -75,7 +87,55 @@ def nf4_roundtrip(weight: torch.Tensor, blocksize: int = 64, double_quant: bool 
         safe2 = torch.where(absmax2 > 0, absmax2, torch.ones_like(absmax2))
         q8 = _nearest(c / safe2[:, None], code8)
         absmax = (code8[q8] * absmax2[:, None]).flatten()[: absmax.numel()] + offset
-    out = (code[q4] * absmax[:, None]).flatten()[:n]
+    return codes, absmax
+
+
+def _unpack(codes: torch.Tensor) -> torch.Tensor:
+    """uint8 [..., n] -> int64 code indices [..., 2n] (high nibble first)."""
+    return torch.stack([codes >> 4, codes & 15], dim=-1).flatten(-2).long()
+
+
+@torch.no_grad()
+def nf4_quantize(weight: torch.Tensor, double_quant: bool = True) -> tuple[torch.Tensor, torch.Tensor]:
+    """``quantize_4bit`` of one ``[N, K]`` nn.Linear weight (``K % 64 == 0``) in the device format: (codes uint8
+    ``[N, K/2]``, absmax' fp32 ``[K/64, N]``), on ``weight``'s device.  Quantise each checkpoint matrix on its own:
+    the double quantisation's offset is the mean over the whole matrix."""
+    if weight.dim() != 2 or weight.shape[1] % BLOCK:
+        raise ValueError(f'nf4_quantize: need a [N, K] matrix with K % {BLOCK} == 0, got {tuple(weight.shape)}')
+    n, k = weight.shape
+    w = weight.detach().to(torch.float32).reshape(-1, BLOCK)
+    codes, absmax = _quantize_blocks(w, double_quant)
+    del w
+    return codes.view(n, k // 2), absmax.view(n, k // BLOCK).t().contiguous()
+
+
+@torch.no_grad()
+def nf4_dequantize(codes: torch.Tensor, absmax: torch.Tensor) -> torch.Tensor:
+    """Device format -> fp32 ``[N, K]``: ``code[q] * absmax'``, one fp32 product per element."""
+    code = torch.tensor(NF4_CODE, dtype=torch.float32, device=codes.device)
+    return code[_unpack(codes)] * absmax.t().repeat_interleave(BLOCK, dim=1)
+
+
+def nf4_storable(weight: torch.Tensor) -> bool:
+    """Whether :func:`nf4_quantize` takes this matrix (every quantised matrix of a built checkpoint shape does)."""
+    return weight.dim() == 2 and weight.shape[1] % BLOCK == 0
+
+
+@torch.no_grad()
+def nf4_roundtrip(weight: torch.Tensor, blocksize: int = 64, double_quant: bool = True) -> torch.Tensor:
+    """``dequantize_4bit(quantize_4bit(weight))`` as fp32, same shape and device as ``weight``: for a matrix the
+    device format takes, ``nf4_dequantize(*nf4_quantize(weight))``."""
+    if blocksize == BLOCK and nf4_storable(weight):
+        return nf4_dequantize(*nf4_quantize(weight, double_quant))
+    w = weight.detach().to(torch.float32)
+    flat = w.flatten()
+    n = flat.numel()
+    pad = (-n) % blocksize
+    if pad:
+        flat = torch.cat([flat, flat.new_zeros(pad)])
+    codes, absmax = _quantize_blocks(flat.view(-1, blocksize), double_quant)
+    code = torch.tensor(NF4_CODE, dtype=torch.float32, device=w.device)
+    out = (code[_unpack(codes)] * absmax[:, None]).flatten()[:n]
     return out.view_as(w)
 
 
@@ -91,12 +151,18 @@ _LINEAR_SUFFIXES = (
 )
 
 
+def is_quantized_linear(name: str, t: torch.Tensor) -> bool:
+    """A transformer-block ``nn.Linear`` weight: what bitsandbytes stores in NF4 (embeddings, norms and biases are
+    not quantised)."""
+    return name.endswith(_LINEAR_SUFFIXES) and t.dim() == 2
+
+
 def quantize_state_dict_nf4(state_dict: dict[str, torch.Tensor], device: torch.device | str | None = None) -> dict:
-    """Copy of ``state_dict`` whose transformer-block ``nn.Linear`` weights went through NF4 (embeddings, norms
-    and biases are not quantised by bitsandbytes either).  The round trip runs on ``device`` when given."""
+    """Copy of ``state_dict`` whose transformer-block ``nn.Linear`` weights went through the NF4 round trip, as
+    fp32 (the load-time path: what the 16-bit GEMMs see).  The round trip runs on ``device`` when given."""
     out = {}
     for name, t in state_dict.items():
-        if name.endswith(_LINEAR_SUFFIXES) and t.dim() == 2:
+        if is_quantized_linear(name, t):
             src = t.to(device) if device is not None else t
             out[name] = nf4_roundtrip(src)
         else:

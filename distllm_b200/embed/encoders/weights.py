@@ -15,11 +15,19 @@ BERT (``B2E_ARCH_BERT``), 5 + 12*L device tensors:
 Names on the right are HF ``BertModel`` state-dict keys (transformers/models/bert/modeling_bert.py).
 Matrices keep nn.Linear's [out_features, in_features] layout, which is the K-major B operand the
 wgmma GEMM wants, so no transposes are needed.
+
+Every list builder takes ``matrix``: the conversion of ONE checkpoint matrix to its device form.  By default that is
+the build's 16-bit storage type (:func:`to_storage`); :func:`nf4_matrix` gives an :class:`Nf4Matrix` instead
+(``b2e_encoder_create_nf4``).  The layout steps that follow -- row concatenation, the gate/up interleave, zero
+padding -- apply to both forms alike (:func:`cat_rows`, :func:`interleave_gate_up`, :func:`pad_rows`,
+:func:`pad_cols`), so an NF4 slot dequantises to exactly the 16-bit slot.
 """
 
 from __future__ import annotations
 
+from typing import Callable
 from typing import Mapping
+from typing import NamedTuple
 
 import torch
 
@@ -37,6 +45,77 @@ def to_storage(t: torch.Tensor, device: torch.device, dtype: torch.dtype) -> tor
     if dtype == torch.float16:
         x = x.clamp(-HALF_MAX, HALF_MAX)
     return x.to(dtype).contiguous()
+
+
+class Nf4Matrix(NamedTuple):
+    """One NF4 weight matrix [N, K] in the device format (embed/encoders/nf4.py: nf4_quantize)."""
+
+    codes: torch.Tensor    # uint8 [N, K/2]
+    absmax: torch.Tensor   # fp32 [K/64, N]
+
+
+Matrix = 'torch.Tensor | Nf4Matrix'
+NF4_ZERO = 0x77   # two NF4 codes 7 (0.0): padding, with scale 0
+
+
+def storage_matrix(device: torch.device, dtype: torch.dtype) -> Callable[[torch.Tensor], torch.Tensor]:
+    return lambda t: to_storage(t, device, dtype)
+
+
+def nf4_matrix(device: torch.device) -> Callable[[torch.Tensor], Nf4Matrix]:
+    """Quantise one checkpoint matrix on ``device``: only its fp32 copy and the codes / scales live there."""
+    from distllm_b200.embed.encoders.nf4 import nf4_quantize
+
+    def convert(t: torch.Tensor) -> Nf4Matrix:
+        return Nf4Matrix(*nf4_quantize(t.detach().to(device=device, dtype=torch.float32)))
+
+    return convert
+
+
+def cat_rows(mats: list) -> Matrix:
+    if isinstance(mats[0], Nf4Matrix):
+        return Nf4Matrix(torch.cat([m.codes for m in mats]), torch.cat([m.absmax for m in mats], dim=1))
+    return torch.cat(mats)
+
+
+def row_slice(m: Matrix, start: int, stop: int) -> Matrix:
+    if isinstance(m, Nf4Matrix):
+        return Nf4Matrix(m.codes[start:stop], m.absmax[:, start:stop])
+    return m[start:stop]
+
+
+def pad_rows(m: Matrix, n: int) -> Matrix:
+    """n zero rows below."""
+    if isinstance(m, Nf4Matrix):
+        codes = torch.full((n, m.codes.shape[1]), NF4_ZERO, dtype=torch.uint8, device=m.codes.device)
+        absmax = m.absmax.new_zeros((m.absmax.shape[0], n))
+        return Nf4Matrix(torch.cat([m.codes, codes]), torch.cat([m.absmax, absmax], dim=1))
+    return torch.cat([m, m.new_zeros((n, m.shape[1]))])
+
+
+def pad_cols(m: Matrix, n: int) -> Matrix:
+    """n zero columns on the right (NF4: whole 64-column blocks)."""
+    if isinstance(m, Nf4Matrix):
+        if n % 64:
+            raise ValueError(f'NF4 column padding {n} is not a multiple of 64')
+        codes = torch.full((m.codes.shape[0], n // 2), NF4_ZERO, dtype=torch.uint8, device=m.codes.device)
+        absmax = m.absmax.new_zeros((n // 64, m.absmax.shape[1]))
+        return Nf4Matrix(torch.cat([m.codes, codes], dim=1), torch.cat([m.absmax, absmax]))
+    return torch.cat([m, m.new_zeros((m.shape[0], n))], dim=1)
+
+
+def device_weight_bytes(weights: list) -> dict[str, int]:
+    """Device bytes of a weight list: ``matrix`` (16-bit matrices, or NF4 codes + scales) and ``other`` (fp32
+    embedding tables, norms, biases)."""
+    matrix = other = 0
+    for w in weights:
+        if isinstance(w, Nf4Matrix):
+            matrix += w.codes.nbytes + w.absmax.nbytes
+        elif w.dtype in (torch.float16, torch.bfloat16):
+            matrix += w.nbytes
+        else:
+            other += w.nbytes
+    return {'matrix': matrix, 'other': other}
 
 
 def bert_desc(hf_config) -> _native.ModelDesc:
@@ -70,15 +149,14 @@ def bert_weight_list(
     num_layers: int,
     device: torch.device,
     dtype: torch.dtype = torch.float16,
-) -> list[torch.Tensor]:
+    matrix: Callable[[torch.Tensor], Matrix] | None = None,
+) -> list:
     """HF BertModel state dict -> contiguous device tensors in ABI order."""
     sd = {k[5:] if k.startswith('bert.') else k: v for k, v in state_dict.items()}
+    b16 = matrix or storage_matrix(device, dtype)
 
     def f32(key: str) -> torch.Tensor:
         return sd[key].detach().to(device=device, dtype=torch.float32).contiguous()
-
-    def b16(t: torch.Tensor) -> torch.Tensor:
-        return to_storage(t, device, dtype)
 
     out = [
         f32('embeddings.word_embeddings.weight'),
@@ -89,10 +167,10 @@ def bert_weight_list(
     ]
     for layer in range(num_layers):
         p = f'encoder.layer.{layer}.'
-        qkv_w = torch.cat([sd[p + f'attention.self.{n}.weight'] for n in ('query', 'key', 'value')])
+        qkv_w = cat_rows([b16(sd[p + f'attention.self.{n}.weight']) for n in ('query', 'key', 'value')])
         qkv_b = torch.cat([sd[p + f'attention.self.{n}.bias'] for n in ('query', 'key', 'value')])
         out += [
-            b16(qkv_w),
+            qkv_w,
             qkv_b.detach().to(device=device, dtype=torch.float32).contiguous(),
             b16(sd[p + 'attention.output.dense.weight']),
             f32(p + 'attention.output.dense.bias'),
@@ -320,8 +398,11 @@ def mistral_desc(hf_config) -> _native.ModelDesc:
     )
 
 
-def interleave_gate_up(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
+def interleave_gate_up(gate: Matrix, up: Matrix) -> Matrix:
     """[I,H], [I,H] -> [2I,H] in the block-interleaved row order the SwiGLU epilogue expects."""
+    if isinstance(gate, Nf4Matrix):
+        return Nf4Matrix(interleave_gate_up(gate.codes, up.codes),
+                         interleave_gate_up(gate.absmax.t(), up.absmax.t()).t().contiguous())
     i, h = gate.shape
     if i % GATE_UP_BLOCK:
         raise ValueError(f'intermediate_size {i} must be a multiple of {GATE_UP_BLOCK}')
@@ -335,26 +416,24 @@ def mistral_weight_list(
     num_layers: int,
     device: torch.device,
     dtype: torch.dtype = torch.float16,
-) -> list[torch.Tensor]:
+    matrix: Callable[[torch.Tensor], Matrix] | None = None,
+) -> list:
     """HF MistralModel (or ...ForCausalLM) state dict -> contiguous device tensors in ABI order."""
     sd = {k[6:] if k.startswith('model.') else k: v for k, v in state_dict.items()}
+    b16 = matrix or storage_matrix(device, dtype)
 
     def f32(key: str) -> torch.Tensor:
         return sd[key].detach().to(device=device, dtype=torch.float32).contiguous()
 
-    def b16(t: torch.Tensor) -> torch.Tensor:
-        return to_storage(t, device, dtype)
-
     out = [f32('embed_tokens.weight'), f32('norm.weight')]
     for layer in range(num_layers):
         p = f'layers.{layer}.'
-        qkv = torch.cat([sd[p + f'self_attn.{n}_proj.weight'] for n in ('q', 'k', 'v')])
         out += [
             f32(p + 'input_layernorm.weight'),
-            b16(qkv),
+            cat_rows([b16(sd[p + f'self_attn.{n}_proj.weight']) for n in ('q', 'k', 'v')]),
             b16(sd[p + 'self_attn.o_proj.weight']),
             f32(p + 'post_attention_layernorm.weight'),
-            b16(interleave_gate_up(sd[p + 'mlp.gate_proj.weight'], sd[p + 'mlp.up_proj.weight'])),
+            interleave_gate_up(b16(sd[p + 'mlp.gate_proj.weight']), b16(sd[p + 'mlp.up_proj.weight'])),
             b16(sd[p + 'mlp.down_proj.weight']),
         ]
     return out
@@ -423,10 +502,11 @@ def qwen3_weight_list(
     num_layers: int,
     device: torch.device,
     dtype: torch.dtype = torch.float16,
-) -> list[torch.Tensor]:
+    matrix: Callable[[torch.Tensor], Matrix] | None = None,
+) -> list:
     """HF Qwen3Model (or ...ForCausalLM, ``model.`` prefix) state dict -> contiguous device tensors in ABI order."""
     sd = {k[6:] if k.startswith('model.') else k: v for k, v in state_dict.items()}
-    mistral = mistral_weight_list(sd, num_layers, device, dtype)
+    mistral = mistral_weight_list(sd, num_layers, device, dtype, matrix)
     out = mistral[:2]
     for layer in range(num_layers):
         p = f'layers.{layer}.self_attn.'
@@ -522,10 +602,12 @@ def modernbert_weight_list(
     num_layers: int,
     device: torch.device,
     dtype: torch.dtype = torch.bfloat16,
-) -> list[torch.Tensor]:
+    matrix: Callable[[torch.Tensor], Matrix] | None = None,
+) -> list:
     """HF ModernBertModel (or ...ForMaskedLM) state dict -> contiguous device tensors in ABI order."""
     sd = {k[6:] if k.startswith('model.') else k: v for k, v in state_dict.items()}
     hidden = sd['embeddings.norm.weight'].shape[0]
+    b16 = matrix or storage_matrix(device, dtype)
 
     def f32(key: str, default: float | None = None) -> torch.Tensor:
         if key not in sd:
@@ -534,9 +616,6 @@ def modernbert_weight_list(
             return torch.full((hidden,), default, dtype=torch.float32, device=device)
         return sd[key].detach().to(device=device, dtype=torch.float32).contiguous()
 
-    def b16(t: torch.Tensor) -> torch.Tensor:
-        return to_storage(t, device, dtype)
-
     out = [
         f32('embeddings.tok_embeddings.weight'),
         f32('embeddings.norm.weight'), f32('embeddings.norm.bias', 0.0),
@@ -544,22 +623,21 @@ def modernbert_weight_list(
     ]
     for layer in range(num_layers):
         p = f'layers.{layer}.'
-        wi = sd[p + 'mlp.Wi.weight'].detach().to(device=device, dtype=torch.float32)
-        wo_mlp = sd[p + 'mlp.Wo.weight'].detach().to(device=device, dtype=torch.float32)
-        inter = wi.shape[0] // 2
+        wi = b16(sd[p + 'mlp.Wi.weight'])
+        wo_mlp = b16(sd[p + 'mlp.Wo.weight'])
+        inter = sd[p + 'mlp.Wi.weight'].shape[0] // 2
         pad = modernbert_padded_intermediate(inter) - inter
-        w_in, w_gate = wi[:inter], wi[inter:]
+        w_in, w_gate = row_slice(wi, 0, inter), row_slice(wi, inter, 2 * inter)
         if pad:
-            zeros = torch.zeros((pad, wi.shape[1]), dtype=wi.dtype, device=wi.device)
-            w_in, w_gate = torch.cat([w_in, zeros]), torch.cat([w_gate, zeros])
-            wo_mlp = torch.cat([wo_mlp, torch.zeros((wo_mlp.shape[0], pad), dtype=wo_mlp.dtype, device=device)], dim=1)
+            w_in, w_gate = pad_rows(w_in, pad), pad_rows(w_gate, pad)
+            wo_mlp = pad_cols(wo_mlp, pad)
         out += [
             f32(p + 'attn_norm.weight', 1.0), f32(p + 'attn_norm.bias', 0.0),   # layer 0: Identity (unused)
             b16(sd[p + 'attn.Wqkv.weight']),
             b16(sd[p + 'attn.Wo.weight']),
             f32(p + 'mlp_norm.weight'), f32(p + 'mlp_norm.bias', 0.0),
-            b16(interleave_gate_up(w_in, w_gate)),
-            b16(wo_mlp),
+            interleave_gate_up(w_in, w_gate),
+            wo_mlp,
         ]
     return out
 

@@ -118,6 +118,15 @@ int b2e_num_weights(const B2EModelDesc* desc);
 int b2e_check_model(const B2EModelDesc* desc);
 int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int n_weights,
                        int device, B2EEncoder** out);
+/* The same model with every weight matrix held in 4-bit NF4 (distllm/embed/encoders/auto.py:44-56's default
+ * quantization; distllm_b200/embed/encoders/nf4.py: nf4_quantize): each matrix slot [N,K] of `weights` points to
+ * its codes, uint8 [N, K/2] row-major (byte j of a row: column 2j in the high nibble, 2j+1 in the low one), and
+ * `absmax` holds 4 * num_layers pointers to the fp32 block scales [K/64, N] (16-byte aligned), per layer in the
+ * order Wqkv, Wo, W1 (Mistral / Qwen3: Wgu, ModernBERT: Wi), W2 (Wd, mlp.Wo).  Every GEMM of the handle
+ * dequantises W = round16(code[q] * absmax) into shared memory in front of the tensor cores, so the results equal
+ * bit for bit those of b2e_encoder_create on the dequantised 16-bit matrices. */
+int b2e_encoder_create_nf4(const B2EModelDesc* desc, const void* const* weights, int n_weights,
+                           const float* const* absmax, int n_absmax, int device, B2EEncoder** out);
 void b2e_encoder_destroy(B2EEncoder* enc);
 
 /* Bytes of device workspace the handle holds for a [B,S] batch (grown lazily, never shrunk). */
@@ -157,6 +166,9 @@ int b2e_adjacent_cosine_dist(const void* emb, int dtype, int64_t n_rows, int H,
 /* Building blocks (storage type, row-major, fp32 accumulation): out[M,N] = epi(A[M,K] . W[N,K]^T + bias [+ resid]). */
 int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* resid, void* out,
                   int M, int N, int K, int epilogue, void* stream);
+/* The same with W in NF4: codes uint8 [N, K/2] and fp32 scales absmax [K/64, N] (see b2e_encoder_create_nf4). */
+int b2e_gemm_nf4(const void* A, const void* codes, const float* absmax, const float* bias, const void* resid,
+                 void* out, int M, int N, int K, int epilogue, void* stream);
 /* qkv [B*S, 3*heads*64] -> ctx [B*S, heads*64]; `reserved` must be NULL (it was a debug score dump). */
 int b2e_attention_d64(const void* qkv, const int64_t* attention_mask, void* ctx, int B, int S,
                       int heads, float* reserved, void* stream);
