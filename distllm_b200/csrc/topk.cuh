@@ -6,8 +6,10 @@
 // The scan is HBM-bound for small query batches: every corpus row is read once for up to TOPK_QT
 // queries.  A warp holds TOPK_ROWS rows in registers, streams the query tile from shared memory (one
 // load feeds TOPK_ROWS rows) and keeps one partial dot product per (query, row); candidates that beat the
-// CTA's current k-th score enter a small shared-memory set under a per-query lock (rare after the first
-// few thousand rows).  A second kernel merges the per-CTA sets of one query and sorts the survivors.
+// CTA's current k-th row -- higher score, or an equal score and a lower row id -- enter a small
+// shared-memory set under a per-query lock (rare after the first few thousand rows).  A second kernel
+// merges the per-CTA sets of one query and sorts the survivors.  Equal scores are resolved by row id at
+// every step, so the result does not depend on the order in which warps and CTAs reach the rows.
 #pragma once
 
 #include "common.cuh"
@@ -21,49 +23,84 @@ constexpr int TOPK_QT = 16;        // queries per pass over the corpus (wide var
 constexpr int TOPK_THREADS = 256;
 constexpr int TOPK_MAX_K = 256;
 
-// ---- a k-slot candidate set in shared memory: replace-the-minimum insertion by a whole warp
+// ---- a k-slot candidate set in shared memory: replace-the-worst insertion by a whole warp
+// The set keeps the k best rows in a strict total order: higher score first, then lower row id (the
+// contract's "ties by ascending index").  Which rows it ends up with is therefore independent of the
+// order the rows are offered in: of the lanes' value layout, of warp scheduling, of the merge's walk.
 struct TopkSet {
   float* score;    // [k]
-  int64_t* index;  // [k]
-  float* kth;      // current minimum of the set (threshold for new candidates)
-  int* kth_pos;
+  int64_t* index;  // [k]; -1 = empty slot (score -inf), worse than any row
+  float* kth;      // score of the set's worst slot (threshold for new candidates)
+  int* kth_pos;    // position of the worst slot
   int* lock;
 };
 
-__device__ __noinline__ void topk_insert(const TopkSet& s, int k, float score, int64_t idx, int lane) {
+// row id of a slot as an ordering key: an empty slot's -1 sorts above every row id
+__device__ __forceinline__ int64_t topk_id_key(const TopkSet& s, int slot) {
+  const int64_t idx = reinterpret_cast<volatile int64_t*>(s.index)[slot];
+  return idx < 0 ? INT64_MAX : idx;
+}
+
+__device__ __forceinline__ void topk_insert_inline(const TopkSet& s, int k, float score, int64_t idx, int lane) {
   // all 32 lanes call this together with the same (score, idx); every decision below is taken on lane
-  // 0's reading of the threshold so that the warp never diverges around the __syncwarp()s
+  // 0's reading of the threshold so that the warp never diverges around the __syncwarp()s.  The worst
+  // slot only ever gets better, so a score strictly below any reading of the threshold can be rejected
+  // without the lock; an equal score is decided under the lock by the row ids.
   float th = *reinterpret_cast<volatile float*>(s.kth);
   th = __shfl_sync(0xffffffffu, th, 0);
-  if (!(score > th)) return;
+  if (!(score >= th)) return;
   if (lane == 0) {
     while (atomicCAS(s.lock, 0, 1) != 0) {
     }
   }
   __syncwarp();
   __threadfence_block();
-  th = *reinterpret_cast<volatile float*>(s.kth);
-  th = __shfl_sync(0xffffffffu, th, 0);
-  if (score > th) {
+  int take = 0, pos = 0;
+  if (lane == 0) {
+    th = *reinterpret_cast<volatile float*>(s.kth);
+    pos = *reinterpret_cast<volatile int*>(s.kth_pos);
+    take = score > th || (score == th && idx < topk_id_key(s, pos));
+  }
+  if (__shfl_sync(0xffffffffu, take, 0)) {
     if (lane == 0) {
-      const int pos = *reinterpret_cast<volatile int*>(s.kth_pos);
       s.score[pos] = score;
       s.index[pos] = idx;
     }
     __syncwarp();
     __threadfence_block();
-    // new minimum: every lane scans a strided part of the set
+    // new worst slot (lowest score, then highest id): every lane scans a strided part of the set for the
+    // lowest score and notes whether it holds that score twice
     float m = INFINITY;
     int mp = 0;
+    bool twice = false;
     for (int i = lane; i < k; i += 32) {
       const float v = reinterpret_cast<volatile float*>(s.score)[i];
-      if (v < m) { m = v; mp = i; }
+      if (v < m) { m = v; mp = i; twice = false; } else if (v == m) { twice = true; }
     }
+    const float lane_min = m;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       const float om = __shfl_xor_sync(0xffffffffu, m, o);
       const int op = __shfl_xor_sync(0xffffffffu, mp, o);
       if (om < m || (om == m && op < mp)) { m = om; mp = op; }
+    }
+    // several slots at the lowest score (duplicate rows, or the empty slots while the set fills): the
+    // worst of them is the highest row id, found in a second pass that only such ties pay for
+    const bool at_min = lane_min == m;
+    if (__popc(__ballot_sync(0xffffffffu, at_min)) > 1 || __any_sync(0xffffffffu, at_min && twice)) {
+      uint64_t key = 0;   // id + 1 of the lane's worst slot at score m (empty slot: all ones); 0 = none
+      int wp = k;
+      for (int i = lane; i < k; i += 32) {
+        if (reinterpret_cast<volatile float*>(s.score)[i] == m) {
+          const uint64_t ki = static_cast<uint64_t>(topk_id_key(s, i)) + 1u;   // INT64_MAX + 1: empty
+          if (ki > key) { key = ki; wp = i; }
+        }
+      }
+      const unsigned hi = __reduce_max_sync(0xffffffffu, static_cast<unsigned>(key >> 32));
+      const unsigned lo = __reduce_max_sync(0xffffffffu, static_cast<unsigned>(key >> 32) == hi
+                                                             ? static_cast<unsigned>(key) : 0u);
+      const bool worst = static_cast<unsigned>(key >> 32) == hi && static_cast<unsigned>(key) == lo;
+      mp = static_cast<int>(__reduce_min_sync(0xffffffffu, worst ? static_cast<unsigned>(wp) : 0xffffffffu));
     }
     if (lane == 0) {
       *reinterpret_cast<volatile int*>(s.kth_pos) = mp;
@@ -74,6 +111,11 @@ __device__ __noinline__ void topk_insert(const TopkSet& s, int k, float score, i
   __threadfence_block();
   if (lane == 0) atomicExch(s.lock, 0);
   __syncwarp();
+}
+
+// the scan's copy: one out-of-line body shared by all its call sites (see the candidate loop below)
+__device__ __noinline__ void topk_insert(const TopkSet& s, int k, float score, int64_t idx, int lane) {
+  topk_insert_inline(s, k, score, idx, lane);
 }
 
 // One 16-byte vector of a corpus row per lane: 4 fp32 or 8 bf16 elements.
@@ -192,14 +234,15 @@ topk_scan_kernel(const float* __restrict__ queries,   // [nq, H] (this pass's qu
         v[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
       }
     }
-    // the few candidates that beat their query's current k-th score are inserted one by one; the loop
-    // body exists once (64 inlined copies of it used to push the kernel out of the instruction cache)
+    // the few candidates that reach their query's current k-th score are inserted one by one (a score
+    // equal to it may still win on the row id: topk_insert decides); the loop body exists once (64 inlined
+    // copies of it used to push the kernel out of the instruction cache)
 #pragma unroll
     for (int j = 0; j < PER; ++j) {
       const int my_i = lane * PER + j;
       const int my_q = my_i / TOPK_ROWS, my_r = my_i % TOPK_ROWS;
       const float th = (my_q < nq) ? *reinterpret_cast<volatile float*>(kth + my_q) : INFINITY;
-      const bool cand = (my_q < nq) && (row0 + my_r < N) && (v[j] > th);
+      const bool cand = (my_q < nq) && (row0 + my_r < N) && (v[j] >= th);
       unsigned todo = __ballot_sync(0xffffffffu, cand);
       while (todo != 0) {
         const int src = __ffs(todo) - 1;
@@ -244,13 +287,14 @@ topk_merge_kernel(const float* __restrict__ part_score, const int64_t* __restric
   __syncthreads();
   const TopkSet set{s_score, s_index, &s_kth, &s_kth_pos, &s_lock};
   const int total = parts * k;
-  // warp-uniform candidate per iteration: each warp walks its own slice
+  // warp-uniform candidate per iteration: each warp walks its own slice (in any order: topk_insert keeps
+  // the k best by (score, row id))
   const int warp = threadIdx.x >> 5;
   for (int c = warp; c < total; c += TOPK_THREADS / 32) {
     const int part = c / k, slot = c % k;
     const size_t off = (static_cast<size_t>(part) * nq + q) * k + slot;
     const int64_t idx = part_index[off];
-    if (idx >= 0) topk_insert(set, k, part_score[off], idx, lane);
+    if (idx >= 0) topk_insert_inline(set, k, part_score[off], idx, lane);
   }
   __syncthreads();
   // bitonic sort of TOPK_MAX_K slots (slots >= k hold -inf / -1)
