@@ -90,6 +90,8 @@ DEBUG_EXPORTS = (
     'b2e_debug_set_layers',
     'b2e_debug_set_att3_variant',
     'b2e_debug_set_packing',
+    'b2e_debug_set_gemm_bn',
+    'b2e_debug_gemm_bn',
     'b2e_debug_topk_tc_fell_back',
 )
 

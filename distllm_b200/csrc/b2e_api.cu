@@ -197,16 +197,41 @@ int check_gemm_shape(int M, int N, int K) {
 
 bool g_gemm_profiling = false;   // b2e_debug_set_clock_buffer: the bias GEMM runs its timeline instantiation
 
-// The W operand of a GEMM: a 16-bit [N,K] map (box 64 x GEMM_BN), or with absmax set the NF4 code map
-// (make_tmap_codes) and the block scales [K/64, N] it is dequantised with.
+// B2E_GEMM_BN=128 | 192 or b2e_debug_set_gemm_bn forces the GEMM tile width of the W maps built from then on (A/B
+// measurements, the equality tests); 0: the rule of gemm_bn
+int g_gemm_bn = -1;   // -1: not decided yet (B2E_GEMM_BN)
+inline int gemm_bn_override() {
+  if (g_gemm_bn < 0) {
+    const char* e = getenv("B2E_GEMM_BN");
+    const int v = e ? atoi(e) : 0;
+    g_gemm_bn = (v == 128 || v == 192) ? v : 0;
+  }
+  return g_gemm_bn;
+}
+
+// The tile width of the GEMM whose W has N rows (gemm.cuh): 192 wherever that kernel exists (16-bit weights, not a
+// gated epilogue) and divides N, else 128.
+int gemm_bn(int N, int epi, bool nf4) {
+  const bool wide_ok = !nf4 && epi != B2E_EPI_SWIGLU && epi != B2E_EPI_GEGLU && N % 192 == 0;
+  if (!wide_ok) return 128;
+  const int forced = gemm_bn_override();
+  return forced ? forced : 192;
+}
+
+// The W operand of a GEMM: a 16-bit [N,K] map (box 64 x bn), or with absmax set the NF4 code map
+// (make_tmap_codes) and the block scales [K/64, N] it is dequantised with.  `bn` is the tile width the map was
+// built for; the launch runs the kernel of that width.
 struct GemmW {
   CUtensorMap tm;
   const float* absmax = nullptr;
+  int bn = GEMM_BN;
 };
 
-int make_gemm_w(GemmW* w, const void* base, const float* absmax, uint64_t rows, uint64_t cols) {
+// epi: the B2E_EPI_* epilogue the GEMM will run with (it decides the tile width with N and the storage)
+int make_gemm_w(GemmW* w, const void* base, const float* absmax, uint64_t rows, uint64_t cols, int epi) {
   w->absmax = absmax;
-  return absmax ? make_tmap_codes(&w->tm, base, rows, cols / 2) : make_tmap_h16(&w->tm, base, rows, cols, GEMM_BN);
+  w->bn = gemm_bn((int)rows, epi, absmax != nullptr);
+  return absmax ? make_tmap_codes(&w->tm, base, rows, cols / 2) : make_tmap_h16(&w->tm, base, rows, cols, w->bn);
 }
 
 template <int EPI>
@@ -214,9 +239,19 @@ int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const flo
                     const h16* resid, int M, int N, int K, cudaStream_t st, const int* m_dev) {
   auto kern = gemm_h16_wgmma_kernel<EPI>;
   int smem = GEMM_SMEM_BYTES;
+  if (N % wb.bn != 0) return fail(B2E_ERR_INVALID, "gemm: N=%d is not a multiple of its W map's tile width %d", N, wb.bn);
   if (wb.absmax) {
     kern = gemm_h16_wgmma_kernel<EPI, false, true>;
     smem = GemmPlan<true>::SMEM_BYTES;
+  } else if (wb.bn == 192) {
+    if constexpr (epi_is_glu(EPI)) {
+      return fail(B2E_ERR_INVALID, "gemm: the gated epilogues run 128-wide tiles only");
+    } else {
+      kern = gemm_h16_wgmma_kernel<EPI, false, false, 192>;
+      smem = GemmPlan<false, 192>::SMEM_BYTES;
+      if constexpr (EPI == EPI_BIAS)
+        if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true, false, 192>;
+    }
   } else if constexpr (EPI == EPI_BIAS) {
     if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true>;
   }
@@ -224,7 +259,7 @@ int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const flo
   if (rc) return rc;
   DeviceInfo dev;
   if ((rc = current_device_info(&dev))) return rc;
-  const long long tiles = (long long)(N / GEMM_BN) * ((M + GEMM_BM - 1) / GEMM_BM);
+  const long long tiles = (long long)(N / wb.bn) * ((M + GEMM_BM - 1) / GEMM_BM);
   if (tiles > 0x7fffffffLL) return fail(B2E_ERR_INVALID, "gemm: %lld output tiles exceed one grid", tiles);
   CUtensorMap tm_out;   // the epilogue's TMA stores: 64-column boxes of 128 rows
   if ((rc = make_tmap_h16(&tm_out, out, M, epi_is_glu(EPI) ? N / 2 : N, GEMM_BM))) return rc;
@@ -979,6 +1014,18 @@ int b2e_debug_set_clock_buffer(void* device_buffer) {
   return B2E_OK;
 }
 
+int b2e_debug_set_gemm_bn(int bn) {
+  if (bn != 0 && bn != 128 && bn != 192) return fail(B2E_ERR_INVALID, "gemm tile width %d: 0, 128 or 192", bn);
+  g_gemm_bn = bn;
+  return B2E_OK;
+}
+
+int b2e_debug_gemm_bn(int n, int epi, int nf4, int* out) {
+  if (!out) return fail(B2E_ERR_INVALID, "null argument");
+  *out = gemm_bn(n, epi, nf4 != 0);
+  return B2E_OK;
+}
+
 // 0: every forward pass keeps the padded [B, S] token layout; 1: pooled passes pack attended tokens (default)
 int b2e_debug_set_packing(int on) {
   g_packing = on ? 1 : 0;
@@ -1086,10 +1133,10 @@ int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_w
   e->tm_wqkv.resize(L); e->tm_wo.resize(L); e->tm_w1.resize(L); e->tm_w2.resize(L);
   for (int l = 0; l < L; ++l) {
     const float* const* s = absmax ? absmax + 4 * l : nullptr;
-    if ((rc = make_gemm_w(&e->tm_wqkv[l], e->Mi(l, 1), s ? s[0] : nullptr, QC, H)) ||
-        (rc = make_gemm_w(&e->tm_wo[l], e->Mi(l, 2), s ? s[1] : nullptr, H, CC)) ||
-        (rc = make_gemm_w(&e->tm_w1[l], e->Mi(l, 4), s ? s[2] : nullptr, 2 * I, H)) ||
-        (rc = make_gemm_w(&e->tm_w2[l], e->Mi(l, 5), s ? s[3] : nullptr, H, I))) {
+    if ((rc = make_gemm_w(&e->tm_wqkv[l], e->Mi(l, 1), s ? s[0] : nullptr, QC, H, B2E_EPI_BIAS)) ||
+        (rc = make_gemm_w(&e->tm_wo[l], e->Mi(l, 2), s ? s[1] : nullptr, H, CC, B2E_EPI_BIAS)) ||
+        (rc = make_gemm_w(&e->tm_w1[l], e->Mi(l, 4), s ? s[2] : nullptr, 2 * I, H, B2E_EPI_SWIGLU)) ||
+        (rc = make_gemm_w(&e->tm_w2[l], e->Mi(l, 5), s ? s[3] : nullptr, H, I, B2E_EPI_BIAS))) {
       delete e;
       return rc;
     }
@@ -1147,10 +1194,10 @@ int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_w
     const void* w1 = mbert ? e->Mb(l, 6) : esm ? e->E(l, 8) : e->L(l, 6);
     const void* w2 = mbert ? e->Mb(l, 7) : esm ? e->E(l, 10) : e->L(l, 8);
     const float* const* s = absmax ? absmax + 4 * l : nullptr;
-    if ((rc = make_gemm_w(&e->tm_wqkv[l], wqkv, s ? s[0] : nullptr, 3 * H, H)) ||
-        (rc = make_gemm_w(&e->tm_wo[l], wo, s ? s[1] : nullptr, H, H)) ||
-        (rc = make_gemm_w(&e->tm_w1[l], w1, s ? s[2] : nullptr, n1, H)) ||
-        (rc = make_gemm_w(&e->tm_w2[l], w2, s ? s[3] : nullptr, H, I))) {
+    if ((rc = make_gemm_w(&e->tm_wqkv[l], wqkv, s ? s[0] : nullptr, 3 * H, H, B2E_EPI_BIAS)) ||
+        (rc = make_gemm_w(&e->tm_wo[l], wo, s ? s[1] : nullptr, H, H, B2E_EPI_BIAS)) ||
+        (rc = make_gemm_w(&e->tm_w1[l], w1, s ? s[2] : nullptr, n1, H, mbert ? B2E_EPI_GEGLU : B2E_EPI_BIAS_GELU)) ||
+        (rc = make_gemm_w(&e->tm_w2[l], w2, s ? s[3] : nullptr, H, I, B2E_EPI_BIAS))) {
       delete e;
       return rc;
     }
@@ -1602,7 +1649,7 @@ int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* re
   CUtensorMap ta;
   GemmW tb;
   if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
-  if ((rc = make_gemm_w(&tb, W, nullptr, N, K))) return rc;
+  if ((rc = make_gemm_w(&tb, W, nullptr, N, K, epi))) return rc;
   return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
 }
 
@@ -1620,7 +1667,7 @@ int b2e_gemm_nf4(const void* A, const void* codes, const float* absmax, const fl
   CUtensorMap ta;
   GemmW tb;
   if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
-  if ((rc = make_gemm_w(&tb, codes, absmax, N, K))) return rc;
+  if ((rc = make_gemm_w(&tb, codes, absmax, N, K, epi))) return rc;
   return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
 }
 

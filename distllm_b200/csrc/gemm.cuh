@@ -1,11 +1,17 @@
 // Persistent, warp-specialised h16 GEMM for sm_90a:  out[M,N] = epi(A[M,K] . W[N,K]^T + bias)
 //
-//   warpgroup 2   TMA producer (one elected lane, 40 registers): for every tile of the CTA, the 128 x 64 A box
-//                 and the 128 x 64 W box of each k-block into a five-stage 128B-swizzled shared-memory ring
-//   warpgroups    two consumers (232 registers each), each owning a whole 128 x 128 output tile: two wgmma
-//   0 and 1       m64n128k16 per k16 step sharing the W descriptor, 128 fp32 accumulators per thread; the
+//   warpgroup 2   TMA producer (one elected lane, 40 registers; 24 at BN = 192): for every tile of the CTA, the
+//                 128 x 64 A box and the BN x 64 W box of each k-block into a 128B-swizzled shared-memory ring of
+//                 five stages (three at BN = 192)
+//   warpgroups    two consumers (232 registers each; 240 at BN = 192), each owning a whole 128 x BN output tile:
+//   0 and 1       two wgmma m64nBNk16 per k16 step sharing the W descriptor, BN fp32 accumulators per thread; the
 //                 epilogue (+bias, erf-GELU | +residual | gated activation) runs on those registers, writes h16
 //                 pairs into the warpgroup's swizzled staging tile and one thread stores it with TMA
+//
+// BN (the tile width) is 128 or 192 (GemmPlan).  A 192-wide tile moves a sixth fewer operand bytes through L2 and
+// shared memory per FLOP than a 128-wide one; each output element sums the same products in the same order at
+// either width, so both give the same bits.  The NF4 producer (one W row per thread of 128) and the gated
+// epilogues (gate and up paired in 64-row blocks of a 128-row W tile) exist at BN = 128 only.
 //
 // One CTA per SM walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tiles fastest, so that the CTAs
 // running together share their A rows in L2); consumer 0 takes the CTA's even-numbered tiles, consumer 1 the
@@ -62,26 +68,32 @@ constexpr int GEMM_NF4_CODE_BYTES = GEMM_BN * GEMM_BK / 2;         // 128 rows x
 constexpr int GEMM_NF4_RAW_BYTES = GEMM_NF4_CODE_BYTES + GEMM_BN * 4;   // + 128 fp32 scales
 
 // Shared-memory plan and register split of one instantiation: [stages][output staging][raw ring][mbarriers]
-// [code table].  The 16-bit plan is the constants above.
-template <bool NF4>
+// [code table].  The 16-bit 128-wide plan is the constants above.  At BN = 192 a stage is 40 KiB and each
+// consumer's staging tile three 16 KiB store boxes, which leaves room for three stages.
+template <bool NF4, int BN = GEMM_BN>
 struct GemmPlan {
-  static constexpr int STAGES = NF4 ? 4 : GEMM_STAGES;
-  static constexpr int OUT_OFFSET = STAGES * GEMM_STAGE_BYTES;
-  static constexpr int RAW_OFFSET = OUT_OFFSET + 2 * 2 * GEMM_OUT_BOX;
+  static_assert(BN == 128 || BN == 192, "tile widths");
+  static_assert(!NF4 || BN == 128, "the NF4 producer writes one W row per thread of its warpgroup");
+  static constexpr int STAGE_BYTES = GEMM_A_BYTES + BN * GEMM_BK * 2;
+  static constexpr int OUT_BOXES = BN / 64;   // 64-column TMA store boxes per tile
+  static constexpr int STAGES = NF4 ? 4 : BN == 192 ? 3 : GEMM_STAGES;
+  static constexpr int OUT_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int RAW_OFFSET = OUT_OFFSET + 2 * OUT_BOXES * GEMM_OUT_BOX;
   static constexpr int BAR_OFFSET = RAW_OFFSET + (NF4 ? GEMM_NF4_RAW * GEMM_NF4_RAW_BYTES : 0);
   // full[STAGES], empty[STAGES], then (NF4) raw_full[GEMM_NF4_RAW]
   static constexpr int TABLE_OFFSET = BAR_OFFSET + 16 * STAGES + (NF4 ? 8 * GEMM_NF4_RAW : 0);
   static constexpr int SMEM_BYTES = TABLE_OFFSET + (NF4 ? 16 * 4 : 0) + 1024;
-  // the dequantising producers need more than the TMA-only producer's 40 registers
-  static constexpr int PRODUCER_REGS = NF4 ? 56 : GEMM_PRODUCER_REGS;
-  static constexpr int CONSUMER_REGS = NF4 ? 224 : GEMM_CONSUMER_REGS;
+  // the dequantising producers need more than the TMA-only producer's 40 registers; 192 fp32 accumulators need
+  // more than 232 in the consumers, which the TMA-only producer's 24 leave them
+  static constexpr int PRODUCER_REGS = NF4 ? 56 : BN == 192 ? 24 : GEMM_PRODUCER_REGS;
+  static constexpr int CONSUMER_REGS = NF4 ? 224 : BN == 192 ? 240 : GEMM_CONSUMER_REGS;
   // setmaxnreg moves registers within what the CTA was launched with (__launch_bounds__(384, 1): 168 per thread);
   // a consumer's increase waits until the producers' decrease has freed enough, so a split beyond it never starts
   static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= GEMM_THREADS * 168, "registers the CTA holds");
   static_assert(SMEM_BYTES <= 232448, "shared memory of one SM");
 };
-static_assert(GemmPlan<false>::SMEM_BYTES == GEMM_SMEM_BYTES && GemmPlan<false>::BAR_OFFSET == GEMM_BAR_OFFSET,
-              "the 16-bit plan");
+static_assert(GemmPlan<false>::SMEM_BYTES == GEMM_SMEM_BYTES && GemmPlan<false>::BAR_OFFSET == GEMM_BAR_OFFSET &&
+              GemmPlan<false>::STAGE_BYTES == GEMM_STAGE_BYTES, "the 16-bit plan");
 
 // bitsandbytes' NF4 code values (embed/encoders/nf4.py: NF4_CODE) as fp32 bit patterns
 __constant__ uint32_t kNf4CodeBits[16] = {
@@ -140,8 +152,9 @@ __device__ long long* g_gemm_clock = nullptr;
 struct GemmTiles {
   int first, stride, count, n_tiles;
 };
+template <int BN>
 __device__ __forceinline__ GemmTiles gemm_tiles(int M, int N) {
-  const int n_tiles = N / GEMM_BN;
+  const int n_tiles = N / BN;
   const int tiles = n_tiles * ((M + GEMM_BM - 1) / GEMM_BM);
   const int first = static_cast<int>(blockIdx.x), stride = static_cast<int>(gridDim.x);
   return {first, stride, first < tiles ? (tiles - 1 - first) / stride + 1 : 0, n_tiles};
@@ -246,16 +259,17 @@ __device__ __forceinline__ void gemm_nf4_producer(const CUtensorMap* tm_a, const
 
 // NF4 = false: W is a 16-bit [N,K] map.  NF4 = true: tm_b is the uint8 code map [N,K/2] (box 32 x 128) and absmax
 // the block scales [K/64, N] (gemm_nf4_producer).
-template <int EPI, bool TL = false, bool NF4 = false>
+template <int EPI, bool TL = false, bool NF4 = false, int BN = GEMM_BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
-                      const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x 128
+                      const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x BN
                       const __grid_constant__ CUtensorMap tm_out,  // out [M,N] (GLU: [M,N/2]) box 64 x 128
                       h16* __restrict__ out, const float* __restrict__ bias, const h16* __restrict__ resid,
                       int M, int N, int K, const int* __restrict__ m_dev, const float* __restrict__ absmax) {
-  using P = GemmPlan<NF4>;
+  using P = GemmPlan<NF4, BN>;
+  static_assert(!epi_is_glu(EPI) || BN == 128, "the gated epilogues pair gate and up within a 128-row W tile");
   if (m_dev != nullptr) M = __ldg(m_dev);   // device-resident row count (packed token layout)
-  const GemmTiles tl = gemm_tiles(M, N);
+  const GemmTiles tl = gemm_tiles<BN>(M, N);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sb = (smem_u32(smem_raw) + 1023u) & ~1023u;   // the swizzled tiles need a 1024-byte aligned base
   const uint32_t full_bar = sb + P::BAR_OFFSET;
@@ -288,16 +302,16 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
       uint32_t phase = 0;
       for (int i = 0; i < tl.count; ++i) {
         const int tile = tl.first + i * tl.stride;
-        const int m0 = (tile / tl.n_tiles) * GEMM_BM, n0 = (tile % tl.n_tiles) * GEMM_BN;
+        const int m0 = (tile / tl.n_tiles) * GEMM_BM, n0 = (tile % tl.n_tiles) * BN;
         for (int kb = 0; kb < kblocks; ++kb, ++n) {
           mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
-          const uint32_t dst = sb + stage * GEMM_STAGE_BYTES;
+          const uint32_t dst = sb + stage * P::STAGE_BYTES;
           const uint32_t fb = full_bar + 8u * stage;
-          mbar_expect_tx(fb, GEMM_STAGE_BYTES);
+          mbar_expect_tx(fb, P::STAGE_BYTES);
           tma_load_2d(dst, &tm_a, fb, kb * GEMM_BK, m0);
           tma_load_2d(dst + GEMM_A_BYTES, &tm_b, fb, kb * GEMM_BK, n0);
           if (TL && clk != nullptr && n < 256) clk[n] = clock64();
-          if (++stage == GEMM_STAGES) { stage = 0; phase ^= 1u; }
+          if (++stage == P::STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
@@ -309,7 +323,7 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   const int t = threadIdx.x & 127;
   const int quad = t & 3;
   const int r_lo = 16 * (t >> 5) + ((t & 31) >> 2);   // row of acc[h][4j + {0,1}] in its 64-row half
-  const uint32_t stg = sb + P::OUT_OFFSET + wg * (2 * GEMM_OUT_BOX);
+  const uint32_t stg = sb + P::OUT_OFFSET + wg * (P::OUT_BOXES * GEMM_OUT_BOX);
   int retired = 0;
   // Turn i (the CTA's i-th tile) belongs to consumer i % 2.  The hand-over into turn i (1 <= i < count) is one
   // arrive by the consumer of turn i - 1 after issuing its main loop and one sync by the consumer of turn i
@@ -317,9 +331,9 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   for (int i = wg; i < tl.count; i += 2) {
     const int tile = tl.first + i * tl.stride;
     const int m0 = (tile / tl.n_tiles) * GEMM_BM, n_blk = tile % tl.n_tiles;
-    float acc[2][64];   // rows [64 h, 64 h + 64) of the tile
+    float acc[2][BN / 2];   // rows [64 h, 64 h + 64) of the tile
 #pragma unroll
-    for (int x = 0; x < 64; ++x) acc[0][x] = acc[1][x] = 0.0f;
+    for (int x = 0; x < BN / 2; ++x) acc[0][x] = acc[1][x] = 0.0f;
     if (i > 0) named_bar_sync(GEMM_BAR_TURN + wg, 256);
     // this tile's k-blocks follow the i * kblocks ones of the earlier turns in the ring
     const int it = i * kblocks;
@@ -328,7 +342,7 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
     int prev = -1;
     for (int kb = 0; kb < kblocks; ++kb) {
       mbar_wait(full_bar + 8u * stage, phase);
-      const uint32_t a_addr = sb + stage * GEMM_STAGE_BYTES;
+      const uint32_t a_addr = sb + stage * P::STAGE_BYTES;
       const uint64_t a0 = make_smem_desc_sw128(a_addr), a1 = make_smem_desc_sw128(a_addr + 64 * 128);
       const uint64_t b_desc = make_smem_desc_sw128(a_addr + GEMM_A_BYTES);
       reg_fence(acc[0]);
@@ -336,8 +350,13 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < GEMM_BK / 16; ++k) {
-        wgmma_64x128_ss(acc[0], a0 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
-        wgmma_64x128_ss(acc[1], a1 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+        if constexpr (BN == 192) {
+          wgmma_64x192_ss(acc[0], a0 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+          wgmma_64x192_ss(acc[1], a1 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+        } else {
+          wgmma_64x128_ss(acc[0], a0 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+          wgmma_64x128_ss(acc[1], a1 + 2u * k, b_desc + 2u * k, (kb | k) != 0);
+        }
       }
       wgmma_commit();
       reg_fence(acc[0]);
@@ -392,9 +411,11 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
                                            8 * j + 2 * quad) = pack_h16x2(v0, v1);
           }
     } else {
-      const int col0 = n_blk * GEMM_BN + 2 * quad;
+      const int col0 = n_blk * BN + 2 * quad;
+      // ascending j: the eight accumulators of group j die as it is written, which makes room for the bias pairs
+      // of the groups ahead
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int j = 0; j < BN / 8; ++j) {
         const float2 b = bias != nullptr ? __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * j))
                                          : make_float2(0.0f, 0.0f);
 #pragma unroll
@@ -433,8 +454,8 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
         if constexpr (epi_is_glu(EPI)) {
           tma_store_2d(&tm_out, stg, n_blk * (GEMM_BN / 2), m0);
         } else {
-          tma_store_2d(&tm_out, stg, n_blk * GEMM_BN, m0);
-          tma_store_2d(&tm_out, stg + GEMM_OUT_BOX, n_blk * GEMM_BN + 64, m0);
+#pragma unroll
+          for (int b = 0; b < P::OUT_BOXES; ++b) tma_store_2d(&tm_out, stg + b * GEMM_OUT_BOX, n_blk * BN + 64 * b, m0);
         }
         tma_store_commit();
       }

@@ -25,6 +25,12 @@ int b2e_debug_set_att3_variant(int variant);
 /* device buffer of 4 x 256 int64 filled with clock64() stamps by CTA (0, 0) of the bias GEMM while set (the
  * timeline instantiation runs instead of the production one); NULL switches it off */
 int b2e_debug_set_clock_buffer(void* device_buffer);
+/* tile width of the GEMM (csrc/gemm.cuh) for the W maps built from now on -- encoder handles created and
+ * b2e_gemm_h16 calls made after it: 128 or 192 forces it wherever the 192-wide kernel exists (16-bit weights, no
+ * gated epilogue, N % 192 == 0), 0 restores the built-in rule.  Also B2E_GEMM_BN=128|192.  A/B measurements only. */
+int b2e_debug_set_gemm_bn(int bn);
+/* *out = the tile width a W map of n rows for epilogue epi (B2E_EPI_*) gets now, NF4 (nf4 != 0) or 16-bit */
+int b2e_debug_gemm_bn(int n, int epi, int nf4, int* out);
 /* 0: keep the padded [B, S] token layout on every path; 1 (default, also B2E_PACKED=1): pooled forward passes run
  * on the attended tokens only (csrc/pack.cuh).  Drops the handle's cached CUDA graphs' validity: call it before
  * b2e_embed_host, not between its batches. */
