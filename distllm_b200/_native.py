@@ -93,6 +93,7 @@ DEBUG_EXPORTS = (
     'b2e_debug_set_gemm_bn',
     'b2e_debug_gemm_bn',
     'b2e_debug_topk_tc_fell_back',
+    'b2e_debug_attention_packed',
 )
 
 
@@ -355,6 +356,26 @@ def attention_causal_d128(
     with torch.cuda.device(qkv.device):
         check(lib.b2e_attention_causal_d128(qkv.data_ptr(), attention_mask.data_ptr(), ctx.data_ptr(),
                                             batch, seq, heads, kv_heads, window, stream_ptr(qkv.device)), lib)
+    return ctx
+
+
+def attention_packed(qkv: torch.Tensor, attention_mask: torch.Tensor, batch: int, seq: int, heads: int,
+                     kv_heads: int, head_dim: int, window: int = 0, causal: bool = False) -> torch.Tensor:
+    """Debug hook: one attention step in the token layout an encoder derives from the mask (csrc/pack.cuh).  With
+    every mask row a non-empty prefix, qkv rows cu[b] + s hold the attended tokens back to back, else qkv is the
+    padded [B*S] layout; ctx comes back in the same layout (rows past the last token untouched: zero)."""
+    lib = load(storage_of(qkv.dtype))
+    _cuda_contig(qkv, 'qkv'), _cuda_contig(attention_mask, 'attention_mask')
+    if qkv.shape[0] != batch * seq:
+        raise NativeError(f'attention_packed: qkv has {qkv.shape[0]} rows, expected B*S = {batch * seq}')
+    i32 = C.c_int
+    lib.b2e_debug_attention_packed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, i32, i32, i32, i32, i32, i32,
+                                               i32, C.c_void_p]
+    ctx = torch.zeros((batch * seq, heads * head_dim), dtype=qkv.dtype, device=qkv.device)
+    with torch.cuda.device(qkv.device):
+        check(lib.b2e_debug_attention_packed(qkv.data_ptr(), attention_mask.data_ptr(), ctx.data_ptr(), batch, seq,
+                                             heads, kv_heads, head_dim, window, int(causal),
+                                             stream_ptr(qkv.device)), lib)
     return ctx
 
 

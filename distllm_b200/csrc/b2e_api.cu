@@ -348,6 +348,49 @@ struct SeqLayout {
   const int* tok_src = nullptr;  // [B * S]
 };
 
+// Device buffers behind a packed SeqLayout (pack_prepare): per-sequence lengths and prefix flags, cu, t_real, and
+// the packed-row -> padded-position map.
+struct PackBuffers {
+  int *len_raw = nullptr, *ok = nullptr, *len = nullptr, *cu = nullptr, *t_real = nullptr, *src = nullptr;
+  size_t cap_b = 0, cap_t = 0;
+  uint64_t gen = 0;   // bumped on every reallocation
+  int device = -1;
+  int ensure(int B, size_t tokens) {
+    int dev = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    if (dev != device) {
+      release();
+      device = dev;
+    }
+    if ((size_t)B > cap_b) {
+      ++gen;
+      cudaFree(len_raw); cudaFree(ok); cudaFree(len); cudaFree(cu); cudaFree(t_real);
+      len_raw = ok = len = cu = t_real = nullptr;
+      cap_b = 0;
+      CUDA_TRY(cudaMalloc(&len_raw, sizeof(int) * B));
+      CUDA_TRY(cudaMalloc(&ok, sizeof(int) * B));
+      CUDA_TRY(cudaMalloc(&len, sizeof(int) * B));
+      CUDA_TRY(cudaMalloc(&cu, sizeof(int) * (B + 1)));
+      CUDA_TRY(cudaMalloc(&t_real, sizeof(int) * 2));
+      cap_b = B;
+    }
+    if (tokens > cap_t) {
+      ++gen;
+      cudaFree(src);
+      src = nullptr;
+      cap_t = 0;
+      CUDA_TRY(cudaMalloc(&src, sizeof(int) * tokens));
+      cap_t = tokens;
+    }
+    return B2E_OK;
+  }
+  void release() {
+    cudaFree(len_raw); cudaFree(ok); cudaFree(len); cudaFree(cu); cudaFree(t_real); cudaFree(src);
+    len_raw = ok = len = cu = t_real = src = nullptr;
+    cap_b = cap_t = 0;
+  }
+};
+
 template <int D, int MODE, int V>
 int launch_attention_kernel(const CUtensorMap& tm, const AttnScratch& sc, void* ctx, int B, int S, int heads,
                             int kv_heads, int window, cudaStream_t st, const SeqLayout& lay) {
@@ -580,6 +623,7 @@ struct DeviceGuard {
 
 thread_local PoolScratch g_pool_scratch;  // for the handle-less standalone poolers
 thread_local AttnScratch g_attn_scratch;  // for the standalone attention op
+thread_local PackBuffers g_pack_scratch;  // for b2e_debug_attention_packed
 
 }  // namespace
 
@@ -601,9 +645,7 @@ struct B2EEncoder {
   PoolScratch pool;
   AttnScratch attn;
   // padding-free token layout of the pooled forward pass (pack.cuh)
-  int *pk_len_raw = nullptr, *pk_ok = nullptr, *pk_len = nullptr, *pk_cu = nullptr, *pk_treal = nullptr,
-      *pk_src = nullptr;
-  size_t pk_cap_b = 0, pk_cap_t = 0;
+  PackBuffers pack;
   // weight operands, one per layer: 16-bit maps, or (b2e_encoder_create_nf4) code maps with their block scales
   std::vector<GemmW> tm_wqkv, tm_wo, tm_w1, tm_w2;
   // host-loop staging
@@ -648,7 +690,7 @@ struct B2EEncoder {
   std::vector<StepGraph> graphs;
   uint64_t ws_gen = 0;        // bumped when the workspace or a staging buffer is reallocated
   uint64_t graphs_stamp = 0;  // buffer_stamp() at the time the cached graphs were captured
-  uint64_t buffer_stamp() const { return ws_gen + pool.gen + attn.gen; }
+  uint64_t buffer_stamp() const { return ws_gen + pool.gen + attn.gen + pack.gen; }
   void drop_graphs() {
     for (auto& g : graphs) cudaGraphExecDestroy(g.exec);
     graphs.clear();
@@ -706,26 +748,8 @@ int ensure_workspace(B2EEncoder* e, int B, int S) {
     CUDA_TRY(cudaMalloc(&e->tok_scale, sizeof(float) * B));
     e->cap_scale = B;
   }
-  if ((size_t)B > e->pk_cap_b) {
-    ++e->ws_gen;
-    cudaFree(e->pk_len_raw); cudaFree(e->pk_ok); cudaFree(e->pk_len); cudaFree(e->pk_cu); cudaFree(e->pk_treal);
-    e->pk_len_raw = e->pk_ok = e->pk_len = e->pk_cu = e->pk_treal = nullptr;
-    e->pk_cap_b = 0;
-    CUDA_TRY(cudaMalloc(&e->pk_len_raw, sizeof(int) * B));
-    CUDA_TRY(cudaMalloc(&e->pk_ok, sizeof(int) * B));
-    CUDA_TRY(cudaMalloc(&e->pk_len, sizeof(int) * B));
-    CUDA_TRY(cudaMalloc(&e->pk_cu, sizeof(int) * (B + 1)));
-    CUDA_TRY(cudaMalloc(&e->pk_treal, sizeof(int) * 2));
-    e->pk_cap_b = B;
-  }
-  if (tokens > e->pk_cap_t) {
-    ++e->ws_gen;
-    cudaFree(e->pk_src);
-    e->pk_src = nullptr;
-    e->pk_cap_t = 0;
-    CUDA_TRY(cudaMalloc(&e->pk_src, sizeof(int) * tokens));
-    e->pk_cap_t = tokens;
-  }
+  int rc;
+  if ((rc = e->pack.ensure(B, tokens))) return rc;
   return e->pool.ensure(B, S, (size_t)B * pool_nsplit(S) * e->desc.hidden);
 }
 
@@ -742,16 +766,15 @@ inline bool packing_enabled() {
 // Token layout of this forward pass (pack.cuh), decided and built ON DEVICE from the mask: attended tokens
 // back to back when every mask row is a non-empty prefix and `enable`, else the identity ([B, S]) layout
 // expressed through the same descriptors.
-int pack_prepare(B2EEncoder* e, const int64_t* mask, int B, int S, bool enable, cudaStream_t st, SeqLayout* lay) {
-  pack_lengths_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, e->pk_len_raw, e->pk_ok, B, S);
-  pack_scan_kernel<<<1, 256, 0, st>>>(e->pk_len_raw, e->pk_ok, e->pk_len, e->pk_cu, e->pk_treal, B, S,
-                                      enable ? 1 : 0);
-  pack_fill_kernel<<<dim3((S + 255) / 256, B), 256, 0, st>>>(e->pk_len, e->pk_cu, e->pk_src, B, S);
+int pack_prepare(PackBuffers& pk, const int64_t* mask, int B, int S, bool enable, cudaStream_t st, SeqLayout* lay) {
+  pack_lengths_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, pk.len_raw, pk.ok, B, S);
+  pack_scan_kernel<<<1, 256, 0, st>>>(pk.len_raw, pk.ok, pk.len, pk.cu, pk.t_real, B, S, enable ? 1 : 0);
+  pack_fill_kernel<<<dim3((S + 255) / 256, B), 256, 0, st>>>(pk.len, pk.cu, pk.src, B, S);
   CUDA_TRY(cudaGetLastError());
-  lay->cu = e->pk_cu;
-  lay->len = e->pk_len;
-  lay->t_real = e->pk_treal;
-  lay->tok_src = e->pk_src;
+  lay->cu = pk.cu;
+  lay->len = pk.len;
+  lay->t_real = pk.t_real;
+  lay->tok_src = pk.src;
   return B2E_OK;
 }
 
@@ -1269,8 +1292,7 @@ void b2e_encoder_destroy(B2EEncoder* e) {
   cudaFree(e->stage_in); cudaFree(e->stage_out);
   cudaFree(e->xres); cudaFree(e->tok_scale); cudaFree(e->rope_cos); cudaFree(e->rope_sin);
   cudaFree(e->rope_cos2); cudaFree(e->rope_sin2);
-  cudaFree(e->pk_len_raw); cudaFree(e->pk_ok); cudaFree(e->pk_len); cudaFree(e->pk_cu); cudaFree(e->pk_treal);
-  cudaFree(e->pk_src);
+  e->pack.release();
   e->drop_graphs();
   e->pool.release();
   e->attn.release();
@@ -1357,7 +1379,7 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
   // Pooled paths run on the padding-free token layout (pack.cuh): only attended tokens go through the GEMMs, norms
   // and attention query tiles; nothing here can observe a padded position.
   SeqLayout lay;
-  if ((rc = pack_prepare(e, mask, B, S, packing_enabled(), st, &lay))) return rc;
+  if ((rc = pack_prepare(e->pack, mask, B, S, packing_enabled(), st, &lay))) return rc;
   if (is_decoder(d.arch)) {
     if ((rc = run_mistral_trunk(e, ids, mask, B, S, st, lay))) return rc;
     if (pool_kind == B2E_POOL_LAST_TOKEN) {
@@ -1743,6 +1765,33 @@ int b2e_attention_causal_d128(const void* qkv, const int64_t* mask, void* ctx, i
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
   return launch_attention_causal_d128(qkv, g_attn_scratch, ctx, B, S, heads, kv_heads, window, st);
+}
+
+// The encoder's attention step in its own token layout: pack_prepare decides the layout from the mask (attended
+// tokens back to back when every row is a non-empty prefix, else the identity layout), then the same launch as the
+// trunks, on tensor maps spanning B*S rows.  qkv / ctx rows are in that layout.
+int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
+                               int kv_heads, int head_dim, int window, int causal, void* stream) {
+  if (!qkv || !mask || !ctx) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  const bool ok = causal ? head_dim == 128 && kv_heads > 0 && heads % kv_heads == 0
+                         : (head_dim == 64 || (head_dim == 32 && window == 0)) && kv_heads == heads;
+  if (B <= 0 || S <= 0 || heads <= 0 || window < 0 || !ok)
+    return fail(B2E_ERR_INVALID, "packed attention: no kernel for B=%d S=%d heads=%d/%d head_dim=%d window=%d "
+                "causal=%d", B, S, heads, kv_heads, head_dim, window, causal);
+  int rc;
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  SeqLayout lay;
+  if ((rc = g_pack_scratch.ensure(B, (size_t)B * S))) return rc;
+  if ((rc = pack_prepare(g_pack_scratch, mask, B, S, true, st, &lay))) return rc;
+  if ((rc = attention_prepare(g_attn_scratch, mask, B, S, st))) return rc;
+  if (causal)
+    return launch_attention_causal_d128(qkv, g_attn_scratch, ctx, B, S, heads, kv_heads, window, st, lay);
+  CUtensorMap tkv;
+  if ((rc = make_tmap_h16(&tkv, qkv, (uint64_t)B * S, (uint64_t)3 * heads * head_dim, AT_KC, head_dim))) return rc;
+  if (window > 0) return launch_attention(tkv, g_attn_scratch, ctx, B, S, heads, st, window, lay);
+  return launch_attention_bidir(tkv, g_attn_scratch, ctx, B, S, heads, head_dim, st, lay);
 }
 
 // ---- exact inner-product top-k (retrieval query path)

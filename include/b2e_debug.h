@@ -7,6 +7,8 @@
 #ifndef B2E_DEBUG_H_
 #define B2E_DEBUG_H_
 
+#include <stdint.h>
+
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -37,6 +39,13 @@ int b2e_debug_gemm_bn(int n, int epi, int nf4, int* out);
 int b2e_debug_set_packing(int on);
 /* *out = 1 when this thread's last b2e_topk_ip_tc call had to fall back to the exact scan (synchronises the device) */
 int b2e_debug_topk_tc_fell_back(int* out);
+/* one attention step as an encoder runs it, in the token layout it derives from the mask (csrc/pack.cuh): with
+ * every mask row a non-empty prefix, qkv and ctx hold the attended tokens back to back (row cu[b] + s), else they
+ * are [B*S] rows in the padded layout.  Both span B*S rows.  causal = 0: bidirectional, head_dim 32 or 64
+ * (kv_heads == heads; window > 0: |q - k| <= window, head_dim 64 only); causal = 1: grouped-query causal,
+ * head_dim 128 (window > 0: q - k < window).  The head_dim-64 kernel is b2e_debug_set_att3_variant's. */
+int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
+                               int kv_heads, int head_dim, int window, int causal, void* stream);
 
 #ifdef __cplusplus
 }
