@@ -286,46 +286,69 @@ int launch_gemm(const CUtensorMap& ta, const GemmW& tb, void* out, const float* 
   return fail(B2E_ERR_INVALID, "unknown epilogue %d", epi);
 }
 
-// Per-forward attention inputs derived from the mask (attention3.cuh): additive key bias rows and
-// the number of 64-key chunks that hold an attended key.
-struct AttnScratch {
-  float* bias = nullptr;   // [B, S_pad]
-  int* kv_chunks = nullptr;  // [B]
-  int* plain_chunks = nullptr;  // [B]  leading fully-attended chunks
-  size_t cap_bias = 0, cap_b = 0;
-  uint64_t gen = 0;   // bumped on every reallocation
-  int device = -1;    // the buffers live on this device; a call from another one starts over
-  int ensure(int B, int S_pad) {
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (dev != device) {
-      release();
-      device = dev;
-      ++gen;
-    }
-    if ((size_t)B * S_pad > cap_bias || (size_t)B > cap_b) ++gen;
-    // pointer nulled and capacity zeroed BEFORE the new allocation: a failed cudaMalloc must not leave
-    // a dangling pointer behind a non-zero capacity
-    if ((size_t)B * S_pad > cap_bias) {
-      cudaFree(bias);
-      bias = nullptr;
-      cap_bias = 0;
-      CUDA_TRY(cudaMalloc(&bias, sizeof(float) * (size_t)B * S_pad));
-      cap_bias = (size_t)B * S_pad;
-    }
-    if ((size_t)B > cap_b) {
-      cudaFree(kv_chunks); cudaFree(plain_chunks);
-      kv_chunks = plain_chunks = nullptr;
-      cap_b = 0;
-      CUDA_TRY(cudaMalloc(&kv_chunks, sizeof(int) * B));
-      CUDA_TRY(cudaMalloc(&plain_chunks, sizeof(int) * B));
-      cap_b = B;
-    }
+// A device buffer of n T that only grows.  grow() frees the old one, nulls the pointer and zeroes the capacity
+// BEFORE the new cudaMalloc: a failed allocation leaves "nothing allocated", never a dangling pointer behind a
+// non-zero capacity that a smaller later call would reuse.  Every reallocation bumps the owner's `gen`: captured
+// CUDA graphs hold these pointers (B2EEncoder::buffer_stamp).  Converts to T* wherever a pointer is expected.
+template <typename T>
+struct DevBuf {
+  T* p = nullptr;
+  size_t cap = 0;
+  operator T*() const { return p; }
+  // zero: fill a new allocation with zeros (buffers that are read before anything writes them)
+  int grow(size_t n, uint64_t& gen, bool zero = false) {
+    if (n <= cap) return B2E_OK;
+    ++gen;
+    release();
+    CUDA_TRY(cudaMalloc(&p, n * sizeof(T)));
+    if (zero) CUDA_TRY(cudaMemset(p, 0, n * sizeof(T)));
+    cap = n;
     return B2E_OK;
   }
   void release() {
-    cudaFree(bias); cudaFree(kv_chunks); cudaFree(plain_chunks);
-    bias = nullptr; kv_chunks = plain_chunks = nullptr; cap_bias = cap_b = 0;
+    cudaFree(p);
+    p = nullptr;
+    cap = 0;
+  }
+};
+
+// Scratch that lives on the calling thread's current device: the encoder's per-pass scratch and the thread-local
+// scratch of the handle-less entry points, which a process may call on more than one device.
+struct DeviceScratch {
+  int device = -1;    // the buffers live on this device
+  uint64_t gen = 0;   // bumped on every reallocation or device change
+};
+
+// A call from another device than the buffers' frees them (Scratch::release) and starts over on this one.
+template <typename Scratch>
+int follow_device(Scratch& s) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  if (dev != s.device) {
+    s.release();
+    s.device = dev;
+    ++s.gen;
+  }
+  return B2E_OK;
+}
+
+// Per-forward attention inputs derived from the mask (attention3.cuh): additive key bias rows and
+// the number of 64-key chunks that hold an attended key.
+struct AttnScratch : DeviceScratch {
+  DevBuf<float> bias;          // [B, S_pad]
+  DevBuf<int> kv_chunks;       // [B]
+  DevBuf<int> plain_chunks;    // [B]  leading fully-attended chunks
+  int ensure(int B, int S_pad) {
+    int rc;
+    if ((rc = follow_device(*this)) || (rc = bias.grow((size_t)B * S_pad, gen)) || (rc = kv_chunks.grow(B, gen)) ||
+        (rc = plain_chunks.grow(B, gen)))
+      return rc;
+    return B2E_OK;
+  }
+  void release() {
+    bias.release();
+    kv_chunks.release();
+    plain_chunks.release();
   }
 };
 
@@ -350,44 +373,21 @@ struct SeqLayout {
 
 // Device buffers behind a packed SeqLayout (pack_prepare): per-sequence lengths and prefix flags, cu, t_real, and
 // the packed-row -> padded-position map.
-struct PackBuffers {
-  int *len_raw = nullptr, *ok = nullptr, *len = nullptr, *cu = nullptr, *t_real = nullptr, *src = nullptr;
-  size_t cap_b = 0, cap_t = 0;
-  uint64_t gen = 0;   // bumped on every reallocation
-  int device = -1;
+struct PackBuffers : DeviceScratch {
+  DevBuf<int> len_raw, ok, len;   // [B]
+  DevBuf<int> cu;                 // [B + 1]
+  DevBuf<int> t_real;             // [2]
+  DevBuf<int> src;                // [tokens]
   int ensure(int B, size_t tokens) {
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (dev != device) {
-      release();
-      device = dev;
-    }
-    if ((size_t)B > cap_b) {
-      ++gen;
-      cudaFree(len_raw); cudaFree(ok); cudaFree(len); cudaFree(cu); cudaFree(t_real);
-      len_raw = ok = len = cu = t_real = nullptr;
-      cap_b = 0;
-      CUDA_TRY(cudaMalloc(&len_raw, sizeof(int) * B));
-      CUDA_TRY(cudaMalloc(&ok, sizeof(int) * B));
-      CUDA_TRY(cudaMalloc(&len, sizeof(int) * B));
-      CUDA_TRY(cudaMalloc(&cu, sizeof(int) * (B + 1)));
-      CUDA_TRY(cudaMalloc(&t_real, sizeof(int) * 2));
-      cap_b = B;
-    }
-    if (tokens > cap_t) {
-      ++gen;
-      cudaFree(src);
-      src = nullptr;
-      cap_t = 0;
-      CUDA_TRY(cudaMalloc(&src, sizeof(int) * tokens));
-      cap_t = tokens;
-    }
+    int rc;
+    if ((rc = follow_device(*this)) || (rc = len_raw.grow(B, gen)) || (rc = ok.grow(B, gen)) ||
+        (rc = len.grow(B, gen)) || (rc = cu.grow((size_t)B + 1, gen)) || (rc = t_real.grow(2, gen)) ||
+        (rc = src.grow(tokens, gen)))
+      return rc;
     return B2E_OK;
   }
   void release() {
-    cudaFree(len_raw); cudaFree(ok); cudaFree(len); cudaFree(cu); cudaFree(t_real); cudaFree(src);
-    len_raw = ok = len = cu = t_real = src = nullptr;
-    cap_b = cap_t = 0;
+    len_raw.release(); ok.release(); len.release(); cu.release(); t_real.release(); src.release();
   }
 };
 
@@ -520,65 +520,23 @@ int check_h(int H) {
 }
 
 // Pool-weight scratch shared by the fused and the standalone poolers.
-struct PoolScratch {
-  int* seq_len = nullptr;  // [B]
-  int* kill = nullptr;     // [S]
-  int* idx = nullptr;      // [B]
-  float* w = nullptr;      // [B,S]
-  float* count = nullptr;  // [B]
-  float* part = nullptr;   // [B,nsplit,H]
-  size_t cap_b = 0, cap_s = 0, cap_bs = 0, cap_part = 0;
-  int device = -1;
-  uint64_t gen = 0;   // bumped on every reallocation (captured CUDA graphs hold these pointers)
-
+struct PoolScratch : DeviceScratch {
+  DevBuf<int> seq_len;    // [B]
+  DevBuf<int> kill;       // [S]
+  DevBuf<int> idx;        // [B]
+  DevBuf<float> w;        // [B,S]
+  DevBuf<float> count;    // [B]
+  DevBuf<float> part;     // [B,nsplit,H]
   int ensure(int B, int S, size_t part_elems) {
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (dev != device) {   // buffers of another device: start over on this one
-      release();
-      device = dev;
-      ++gen;
-    }
-    if ((size_t)B > cap_b || (size_t)S > cap_s || (size_t)B * S > cap_bs || part_elems > cap_part) ++gen;
-    // every branch: free, null the pointers and zero the capacity, THEN allocate (a failed cudaMalloc
-    // leaves "nothing allocated", never a dangling pointer that a smaller later call would reuse)
-    if ((size_t)B > cap_b) {
-      cudaFree(seq_len); cudaFree(idx); cudaFree(count);
-      seq_len = idx = nullptr;
-      count = nullptr;
-      cap_b = 0;
-      CUDA_TRY(cudaMalloc(&seq_len, sizeof(int) * B));
-      CUDA_TRY(cudaMalloc(&idx, sizeof(int) * B));
-      CUDA_TRY(cudaMalloc(&count, sizeof(float) * B));
-      cap_b = B;
-    }
-    if ((size_t)S > cap_s) {
-      cudaFree(kill);
-      kill = nullptr;
-      cap_s = 0;
-      CUDA_TRY(cudaMalloc(&kill, sizeof(int) * S));
-      cap_s = S;
-    }
-    if ((size_t)B * S > cap_bs) {
-      cudaFree(w);
-      w = nullptr;
-      cap_bs = 0;
-      CUDA_TRY(cudaMalloc(&w, sizeof(float) * (size_t)B * S));
-      cap_bs = (size_t)B * S;
-    }
-    if (part_elems > cap_part) {
-      cudaFree(part);
-      part = nullptr;
-      cap_part = 0;
-      CUDA_TRY(cudaMalloc(&part, sizeof(float) * part_elems));
-      cap_part = part_elems;
-    }
+    int rc;
+    if ((rc = follow_device(*this)) || (rc = seq_len.grow(B, gen)) || (rc = kill.grow(S, gen)) ||
+        (rc = idx.grow(B, gen)) || (rc = w.grow((size_t)B * S, gen)) || (rc = count.grow(B, gen)) ||
+        (rc = part.grow(part_elems, gen)))
+      return rc;
     return B2E_OK;
   }
   void release() {
-    cudaFree(seq_len); cudaFree(kill); cudaFree(idx); cudaFree(w); cudaFree(count); cudaFree(part);
-    seq_len = kill = idx = nullptr; w = count = part = nullptr;
-    cap_b = cap_s = cap_bs = cap_part = 0;
+    seq_len.release(); kill.release(); idx.release(); w.release(); count.release(); part.release();
   }
 };
 
@@ -630,18 +588,45 @@ thread_local PackBuffers g_pack_scratch;  // for b2e_debug_attention_packed
 // The decoder family (Mistral, Qwen3): pre-RMSNorm blocks, head_dim-128 grouped-query causal attention, SwiGLU.
 // Qwen3 adds a per-head RMSNorm of q and k before the rotary embedding: two more weight slots per layer.
 inline bool is_decoder(int arch) { return arch == B2E_ARCH_MISTRAL || arch == B2E_ARCH_QWEN3; }
-inline int decoder_layer_slots(int arch) { return arch == B2E_ARCH_QWEN3 ? 8 : 6; }
+
+namespace {
+// The final norm of a family and the tensors it reads
+enum FinalNorm {
+  NORM_POST_LN,   // post-LayerNorm over tmp + hidden (BERT): the last ACTIVE layer's LayerNorm
+  NORM_ADD_LN,    // LayerNorm over the fp32 residual stream xres + tmp (ESM-2, ModernBERT)
+  NORM_ADD_RMS,   // RMSNorm over xres + tmp (Mistral, Qwen3)
+};
+
+// Layers 0..num_layers-1 of a family; leaves what its FinalNorm reads.  `types` is BERT's alone.
+using TrunkFn = int (*)(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t* types, int B, int S,
+                        cudaStream_t st, const SeqLayout& lay);
+
+// One row per B2E_ARCH_*: the weight-slot layout of the ABI (embed/encoders/weights.py), what its linear layers
+// run and its trunk.  Slot of (layer l, offset k) = lead + stride * l + k.
+struct Family {
+  int lead, stride;              // fixed leading slots; slots per layer
+  int wqkv, wo, w1, w2;          // per-layer offsets of the four GEMM weights
+  bool w1_gated;                 // W1 holds 2I rows: two halves interleaved in blocks of 64 (B2E_EPI_SWIGLU/GEGLU)
+  int w1_epi;                    // the epilogue W1's GEMM runs with
+  FinalNorm norm;
+  int norm_g, norm_b;            // the final norm's gain / bias: leading slots, or per-layer offsets of the last
+                                 // active layer (NORM_POST_LN); -1: none
+  TrunkFn trunk;
+};
+const Family* family(int arch);   // null: unknown architecture
+}  // namespace
 
 // ================================================================== encoder handle
 struct B2EEncoder {
   B2EModelDesc desc;
+  const Family* fam = nullptr;
   int full_layers = 0;   // desc.num_layers as created (b2e_debug_set_layers may lower desc.num_layers)
   std::vector<const void*> w;
   int device = 0;
   int sms = 0;
-  // activations (h16)
-  size_t cap_tokens = 0;
-  h16 *hidden = nullptr, *qkv = nullptr, *ctx = nullptr, *tmp = nullptr, *ffn = nullptr;
+  // activations (h16); the pre-norm families' fp32 residual stream; ESM-2's token-dropout scales
+  DevBuf<h16> hidden, qkv, ctx, tmp, ffn;
+  DevBuf<float> xres, tok_scale;
   PoolScratch pool;
   AttnScratch attn;
   // padding-free token layout of the pooled forward pass (pack.cuh)
@@ -649,38 +634,23 @@ struct B2EEncoder {
   // weight operands, one per layer: 16-bit maps, or (b2e_encoder_create_nf4) code maps with their block scales
   std::vector<GemmW> tm_wqkv, tm_wo, tm_w1, tm_w2;
   // host-loop staging
-  int64_t* stage_in = nullptr;
-  size_t stage_cap = 0;
-  float* stage_out = nullptr;
-  size_t stage_out_cap = 0;
+  DevBuf<int64_t> stage_in;
+  DevBuf<float> stage_out;
   cudaStream_t own_stream = nullptr;
-
-  // BERT weight slots
-  const float* word() const { return (const float*)w[0]; }
-  const float* pos() const { return (const float*)w[1]; }
-  const float* type() const { return (const float*)w[2]; }
-  const float* emb_g() const { return (const float*)w[3]; }
-  const float* emb_b() const { return (const float*)w[4]; }
-  const void* L(int l, int k) const { return w[5 + 12 * l + k]; }
-
-  // ESM-2: fp32 residual stream, token-dropout scales, rotary tables; weight slots (weights.py):
-  //   0 word emb, 1/2 final LayerNorm; per layer (3 + 12 l): ln1 g/b, Wqkv, bqkv, Wo, bo, ln2 g/b,
-  //   W1, b1, W2, b2
-  float* xres = nullptr;
-  float* tok_scale = nullptr;
-  size_t cap_scale = 0;
+  // rotary tables (make_rope_tables); ModernBERT: rope_cos/sin = full-attention layers' table, rope_cos2/sin2 =
+  // sliding-attention layers'
   float *rope_cos = nullptr, *rope_sin = nullptr;
-  const void* E(int l, int k) const { return w[3 + 12 * l + k]; }
-
-  // Mistral family: fp32 residual stream and rotary tables as above; weight slots (weights.py):
-  //   0 embed_tokens, 1 final norm; per layer (2 + 6 l): input norm, Wqkv, Wo, post-attention norm,
-  //   Wgu (gate/up interleaved), Wd; Qwen3 (2 + 8 l): the same six, then q_norm, k_norm (fp32 [128])
-  const void* Mi(int l, int k) const { return w[2 + decoder_layer_slots(desc.arch) * l + k]; }
-  // ModernBERT: weight slots (weights.py): 0 tok_embeddings, 1/2 embeddings.norm g/b, 3/4 final_norm g/b; per
-  // layer (5 + 8 l): attn_norm g/b, Wqkv, Wo, mlp_norm g/b, Wi (input/gate interleaved), mlp.Wo.  rope_cos/sin =
-  // full-attention layers' table, rope_cos2/sin2 = sliding-attention layers'
-  const void* Mb(int l, int k) const { return w[5 + 8 * l + k]; }
   float *rope_cos2 = nullptr, *rope_sin2 = nullptr;
+
+  // weight slot k of layer l (Family)
+  const void* slot(int l, int k) const { return w[fam->lead + fam->stride * l + k]; }
+  // The final norm's gain (k = 0) and bias (k = 1; null for RMSNorm).  BERT's live in the last active layer, which
+  // b2e_debug_set_layers moves.
+  const float* final_norm(int k) const {
+    const int s = k ? fam->norm_b : fam->norm_g;
+    if (s < 0) return nullptr;
+    return (const float*)(fam->norm == NORM_POST_LN ? slot(desc.num_layers - 1, s) : w[s]);
+  }
   // b2e_embed_host replays one CUDA graph per (batch shape, pooling, staging slot) instead of ~90
   // launches per batch; every graph is dropped when a buffer it points into is reallocated
   struct StepGraph {
@@ -712,43 +682,18 @@ size_t tokens_bytes(const B2EModelDesc& d, size_t tokens) {
 }
 
 int ensure_workspace(B2EEncoder* e, int B, int S) {
-  const size_t tokens = (size_t)B * S;
-  if (tokens > e->cap_tokens) {
-    ++e->ws_gen;
-    cudaFree(e->hidden); cudaFree(e->qkv); cudaFree(e->ctx); cudaFree(e->tmp); cudaFree(e->ffn);
-    e->hidden = e->qkv = e->ctx = e->tmp = e->ffn = nullptr;
-    e->cap_tokens = 0;
-    const size_t H = e->desc.hidden, I = e->desc.intermediate;
-    CUDA_TRY(cudaMalloc(&e->hidden, tokens * H * 2));
-    CUDA_TRY(cudaMalloc(&e->qkv, tokens * (size_t)e->qkv_cols() * 2));
-    CUDA_TRY(cudaMalloc(&e->ctx, tokens * (size_t)e->ctx_cols() * 2));
-    CUDA_TRY(cudaMalloc(&e->tmp, tokens * H * 2));
-    CUDA_TRY(cudaMalloc(&e->ffn, tokens * I * 2));
-    // zeroed once: with the packed token layout rows behind the last attended token are never written by a
-    // forward pass but ARE read (partial GEMM tiles, the last key chunk of the last sequence) -- they must
-    // hold finite values, never whatever the allocator left there
-    CUDA_TRY(cudaMemset(e->hidden, 0, tokens * H * 2));
-    CUDA_TRY(cudaMemset(e->qkv, 0, tokens * (size_t)e->qkv_cols() * 2));
-    CUDA_TRY(cudaMemset(e->ctx, 0, tokens * (size_t)e->ctx_cols() * 2));
-    CUDA_TRY(cudaMemset(e->tmp, 0, tokens * H * 2));
-    CUDA_TRY(cudaMemset(e->ffn, 0, tokens * I * 2));
-    if (e->has_xres()) {
-      cudaFree(e->xres);
-      e->xres = nullptr;
-      CUDA_TRY(cudaMalloc(&e->xres, tokens * H * 4));
-      CUDA_TRY(cudaMemset(e->xres, 0, tokens * H * 4));
-    }
-    e->cap_tokens = tokens;
-  }
-  if (e->desc.arch == B2E_ARCH_ESM2 && (size_t)B > e->cap_scale) {
-    ++e->ws_gen;
-    cudaFree(e->tok_scale);
-    e->tok_scale = nullptr;
-    e->cap_scale = 0;
-    CUDA_TRY(cudaMalloc(&e->tok_scale, sizeof(float) * B));
-    e->cap_scale = B;
-  }
+  const size_t tokens = (size_t)B * S, H = e->desc.hidden, I = e->desc.intermediate;
+  uint64_t& gen = e->ws_gen;
+  // zero-filled on allocation: with the packed token layout rows behind the last attended token are never written
+  // by a forward pass but ARE read (partial GEMM tiles, the last key chunk of the last sequence) -- they must
+  // hold finite values, never whatever the allocator left there
   int rc;
+  if ((rc = e->hidden.grow(tokens * H, gen, true)) || (rc = e->tmp.grow(tokens * H, gen, true)) ||
+      (rc = e->qkv.grow(tokens * e->qkv_cols(), gen, true)) || (rc = e->ctx.grow(tokens * e->ctx_cols(), gen, true)) ||
+      (rc = e->ffn.grow(tokens * I, gen, true)))
+    return rc;
+  if (e->has_xres() && (rc = e->xres.grow(tokens * H, gen, true))) return rc;
+  if (e->desc.arch == B2E_ARCH_ESM2 && (rc = e->tok_scale.grow(B, gen))) return rc;
   if ((rc = e->pack.ensure(B, tokens))) return rc;
   return e->pool.ensure(B, S, (size_t)B * pool_nsplit(S) * e->desc.hidden);
 }
@@ -789,49 +734,65 @@ int validate_batch(const B2EEncoder* e, int B, int S) {
   return B2E_OK;
 }
 
+// The GEMM A operands over the activations of a [B*S] pass (box 128 rows) and, for the bidirectional trunks, the
+// attention operand qkv (box AT_KC x head_dim; the decoders' launch_attention_causal_d128 maps qkv itself).
+struct TrunkMaps {
+  CUtensorMap hidden, ctx, ffn, qkv;
+};
+
+// Every trunk's step after its embedding: attention_prepare for this batch's mask, then the tensor maps.
+int trunk_prologue(B2EEncoder* e, const int64_t* mask, int B, int S, cudaStream_t st, TrunkMaps* tm) {
+  const B2EModelDesc& d = e->desc;
+  const int M = B * S;
+  int rc;
+  if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
+  if ((rc = make_tmap_h16(&tm->hidden, e->hidden, M, d.hidden, 128))) return rc;
+  if ((rc = make_tmap_h16(&tm->ctx, e->ctx, M, e->ctx_cols(), 128))) return rc;
+  if ((rc = make_tmap_h16(&tm->ffn, e->ffn, M, d.intermediate, 128))) return rc;
+  if (is_decoder(d.arch)) return B2E_OK;
+  return make_tmap_h16(&tm->qkv, e->qkv, M, e->qkv_cols(), AT_KC, d.head_dim);
+}
+
 // Layers 0..L-1 up to (and including) the last FFN-down GEMM: leaves the pre-LayerNorm residual sum
 // of the final layer split as e->tmp (FFN-down output + bias) and e->hidden (the residual it still has
 // to be added to); every earlier LayerNorm output lives in e->hidden.
 int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t* types,
-                   int B, int S, cudaStream_t st,
-                   const SeqLayout& lay = SeqLayout()) {
+                   int B, int S, cudaStream_t st, const SeqLayout& lay) {
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate;
   int rc;
+  // leading slots: word, position, token-type embeddings, embedding LayerNorm g/b
   DISPATCH_H(H, (embed_layernorm_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     ids, types, e->word(), e->pos(), e->type(), e->emb_g(), e->emb_b(), e->hidden,
-                     M, S, d.eps, lay.t_real, lay.tok_src)));
+                     ids, types, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2],
+                     (const float*)e->w[3], (const float*)e->w[4], e->hidden, M, S, d.eps, lay.t_real,
+                     lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
 
-  if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv;
-  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, AT_KC, d.head_dim))) return rc;
-  if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
+  TrunkMaps tm;
+  if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
 
   for (int l = 0; l < d.num_layers; ++l) {
-    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, (const float*)e->L(l, 1), nullptr, M,
+    if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, (const float*)e->slot(l, 1), nullptr, M,
                           3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    if ((rc = launch_attention_bidir(tm_qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
+    if ((rc = launch_attention_bidir(tm.qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
       return rc;
     // the residual add rides on the LayerNorm's coalesced reads, not on the GEMM epilogue
-    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, (const float*)e->L(l, 3), nullptr, M, H, H,
+    if ((rc = launch_gemm(tm.ctx, e->tm_wo[l], e->tmp, (const float*)e->slot(l, 3), nullptr, M, H, H,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                       e->tmp, e->hidden, (const float*)e->L(l, 4), (const float*)e->L(l, 5),
+                       e->tmp, e->hidden, (const float*)e->slot(l, 4), (const float*)e->slot(l, 5),
                        e->hidden, M, d.eps, lay.t_real)));
-    if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, (const float*)e->L(l, 7), nullptr, M, I,
+    if ((rc = launch_gemm(tm.hidden, e->tm_w1[l], e->ffn, (const float*)e->slot(l, 7), nullptr, M, I,
                           H, B2E_EPI_BIAS_GELU, st, lay.t_real)))
       return rc;
-    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, (const float*)e->L(l, 9), nullptr, M, H, I,
+    if ((rc = launch_gemm(tm.ffn, e->tm_w2[l], e->tmp, (const float*)e->slot(l, 9), nullptr, M, H, I,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < d.num_layers) {
       DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->tmp, e->hidden, (const float*)e->L(l, 10), (const float*)e->L(l, 11),
+                         e->tmp, e->hidden, (const float*)e->slot(l, 10), (const float*)e->slot(l, 11),
                          e->hidden, M, d.eps, lay.t_real)));
     }
   }
@@ -844,8 +805,8 @@ int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
 // residual stream e->xres stays fp32; each add_layernorm call folds the previous GEMM output into it
 // and emits the next GEMM's h16 input.  Leaves xres (before the last FFN output is added) and e->tmp
 // (that FFN-down output): the caller applies emb_layer_norm_after to xres + tmp.
-int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B, int S,
-                  cudaStream_t st, const SeqLayout& lay = SeqLayout()) {
+int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t*, int B, int S,
+                  cudaStream_t st, const SeqLayout& lay) {
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   const int mask_token = d.reserved - 1;  // reserved = mask_token_id + 1, 0 = token dropout off
@@ -855,19 +816,15 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
                      ids, mask, (const float*)e->w[0], e->tok_scale, e->xres, M, S, mask_token, lay.t_real,
                      lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
-  if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_qkv;
-  if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_qkv, e->qkv, M, 3 * H, AT_KC, d.head_dim))) return rc;
+  TrunkMaps tm;
+  if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
 
   DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     e->xres, nullptr, (const float*)e->E(0, 0), (const float*)e->E(0, 1), e->hidden,
+                     e->xres, nullptr, (const float*)e->slot(0, 0), (const float*)e->slot(0, 1), e->hidden,
                      M, d.eps, lay.t_real)));
   const long long rope_work = (long long)M * d.heads * 2;
   for (int l = 0; l < L; ++l) {
-    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, (const float*)e->E(l, 3), nullptr, M,
+    if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, (const float*)e->slot(l, 3), nullptr, M,
                           3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (d.head_dim == 32) {   // two threads per head of 2 x 16 frequencies
@@ -877,23 +834,23 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
       rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
           e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
     }
-    if ((rc = launch_attention_bidir(tm_qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
+    if ((rc = launch_attention_bidir(tm.qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
       return rc;
-    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, (const float*)e->E(l, 5), nullptr, M, H, H,
+    if ((rc = launch_gemm(tm.ctx, e->tm_wo[l], e->tmp, (const float*)e->slot(l, 5), nullptr, M, H, H,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                       e->xres, e->tmp, (const float*)e->E(l, 6), (const float*)e->E(l, 7), e->hidden,
+                       e->xres, e->tmp, (const float*)e->slot(l, 6), (const float*)e->slot(l, 7), e->hidden,
                        M, d.eps, lay.t_real)));
-    if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, (const float*)e->E(l, 9), nullptr, M, I, H,
+    if ((rc = launch_gemm(tm.hidden, e->tm_w1[l], e->ffn, (const float*)e->slot(l, 9), nullptr, M, I, H,
                           B2E_EPI_BIAS_GELU, st, lay.t_real)))
       return rc;
-    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, (const float*)e->E(l, 11), nullptr, M, H, I,
+    if ((rc = launch_gemm(tm.ffn, e->tm_w2[l], e->tmp, (const float*)e->slot(l, 11), nullptr, M, H, I,
                           B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
       DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, (const float*)e->E(l + 1, 0), (const float*)e->E(l + 1, 1),
+                         e->xres, e->tmp, (const float*)e->slot(l + 1, 0), (const float*)e->slot(l + 1, 1),
                          e->hidden, M, d.eps, lay.t_real)));
     }
   }
@@ -907,8 +864,8 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B,
 // added) and e->tmp (that down_proj output); the caller applies the final norm to xres + tmp.
 // Qwen3 (transformers/models/qwen3/modeling_qwen3.py) is the same block with q_norm / k_norm applied to every q
 // and k head before the rotary embedding: qk_rmsnorm_rope_kernel takes rope_halves_kernel<64>'s place.
-int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B, int S,
-                      cudaStream_t st, const SeqLayout& lay = SeqLayout()) {
+int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t*, int B, int S,
+                      cudaStream_t st, const SeqLayout& lay) {
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   const int QC = e->qkv_cols(), CC = e->ctx_cols();
@@ -916,22 +873,19 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
   DISPATCH_H(H, (mistral_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      ids, (const float*)e->w[0], e->xres, M, lay.t_real, lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
-  if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn;
-  if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, CC, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
+  TrunkMaps tm;
+  if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
 
   DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     e->xres, nullptr, (const float*)e->Mi(0, 0), e->hidden, M, d.eps, lay.t_real)));
+                     e->xres, nullptr, (const float*)e->slot(0, 0), e->hidden, M, d.eps, lay.t_real)));
   const int n_rot = d.heads + d.kv_heads;   // q heads and k heads are adjacent columns of qkv
   const long long rope_work = (long long)M * n_rot;
   for (int l = 0; l < L; ++l) {
-    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, QC, H, B2E_EPI_BIAS, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, QC, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (d.arch == B2E_ARCH_QWEN3) {
       qk_rmsnorm_rope_kernel<<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
-          e->qkv, (const float*)e->Mi(l, 6), (const float*)e->Mi(l, 7), e->rope_cos, e->rope_sin, M, S, d.heads,
+          e->qkv, (const float*)e->slot(l, 6), (const float*)e->slot(l, 7), e->rope_cos, e->rope_sin, M, S, d.heads,
           d.kv_heads, QC, d.eps, lay.t_real, lay.tok_src);
     } else {
       rope_halves_kernel<64><<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
@@ -940,19 +894,19 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
     if ((rc = launch_attention_causal_d128(e->qkv, e->attn, e->ctx, B, S, d.heads, d.kv_heads,
                                            d.sliding_window, st, lay)))
       return rc;
-    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, CC, B2E_EPI_BIAS, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, CC, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                       e->xres, e->tmp, (const float*)e->Mi(l, 3), e->hidden, M, d.eps, lay.t_real)));
+                       e->xres, e->tmp, (const float*)e->slot(l, 3), e->hidden, M, d.eps, lay.t_real)));
     // gate and up in one GEMM (interleaved rows), silu(gate) * up in its epilogue: [M, I]
-    if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H,
+    if ((rc = launch_gemm(tm.hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H,
                           B2E_EPI_SWIGLU, st, lay.t_real)))
       return rc;
-    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
       DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, (const float*)e->Mi(l + 1, 0), e->hidden, M, d.eps, lay.t_real)));
+                         e->xres, e->tmp, (const float*)e->slot(l + 1, 0), e->hidden, M, d.eps, lay.t_real)));
     }
   }
   CUDA_TRY(cudaGetLastError());
@@ -964,8 +918,8 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, in
 // :52-71 (embeddings), :232-310 (attention), :74-91 (MLP), :313-343 (block; layer 0 has no attn_norm),
 // :424-490 (model).  Leaves xres (before the last MLP output is added) and e->tmp (that output): the caller
 // applies final_norm to xres + tmp.
-int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, int B, int S,
-                         cudaStream_t st, const SeqLayout& lay = SeqLayout()) {
+int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t*, int B, int S,
+                         cudaStream_t st, const SeqLayout& lay) {
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   int rc;
@@ -973,38 +927,106 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
                      ids, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2], e->xres,
                      e->hidden, M, d.eps, lay.t_real, lay.tok_src)));
   CUDA_TRY(cudaGetLastError());
-  if ((rc = attention_prepare(e->attn, mask, B, S, st))) return rc;
-  CUtensorMap tm_hidden, tm_ctx, tm_ffn, tm_kv64;
-  if ((rc = make_tmap_h16(&tm_hidden, e->hidden, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ctx, e->ctx, M, H, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_ffn, e->ffn, M, I, 128))) return rc;
-  if ((rc = make_tmap_h16(&tm_kv64, e->qkv, M, 3 * H, AT_KC))) return rc;
+  TrunkMaps tm;
+  if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
   const long long rope_work = (long long)M * d.heads * 2;
   for (int l = 0; l < L; ++l) {
     const bool global = (l % d.global_every) == 0;
     if (l > 0) {
       DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, (const float*)e->Mb(l, 0), (const float*)e->Mb(l, 1), e->hidden, M,
+                         e->xres, e->tmp, (const float*)e->slot(l, 0), (const float*)e->slot(l, 1), e->hidden, M,
                          d.eps, lay.t_real)));
     }
-    if ((rc = launch_gemm(tm_hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, 3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, 3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
         e->qkv, global ? e->rope_cos : e->rope_cos2, global ? e->rope_sin : e->rope_sin2, M, S, 2 * d.heads,
         3 * H, lay.t_real, lay.tok_src);
-    if ((rc = launch_attention(tm_kv64, e->attn, e->ctx, B, S, d.heads, st,
+    if ((rc = launch_attention(tm.qkv, e->attn, e->ctx, B, S, d.heads, st,
                                global ? 0 : d.sliding_window, lay)))
       return rc;
-    if ((rc = launch_gemm(tm_ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, H, B2E_EPI_BIAS, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                       e->xres, e->tmp, (const float*)e->Mb(l, 4), (const float*)e->Mb(l, 5), e->hidden, M,
+                       e->xres, e->tmp, (const float*)e->slot(l, 4), (const float*)e->slot(l, 5), e->hidden, M,
                        d.eps, lay.t_real)));
     // Wi with its input / gate halves interleaved: gelu(input) * gate in the epilogue -> [M, I]
-    if ((rc = launch_gemm(tm_hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H, B2E_EPI_GEGLU, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H, B2E_EPI_GEGLU, st, lay.t_real)))
       return rc;
-    if ((rc = launch_gemm(tm_ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
+    if ((rc = launch_gemm(tm.ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
+}
+
+// Weight slots (embed/encoders/weights.py):
+//   BERT        0 word, 1 position, 2 token-type embeddings, 3/4 embedding LayerNorm g/b; per layer (5 + 12 l):
+//               Wqkv, bqkv, Wo, bo, attention LayerNorm g/b, W1, b1, W2, b2, output LayerNorm g/b
+//   ESM-2       0 word emb, 1/2 final LayerNorm; per layer (3 + 12 l): ln1 g/b, Wqkv, bqkv, Wo, bo, ln2 g/b, W1, b1,
+//               W2, b2
+//   Mistral     0 embed_tokens, 1 final norm; per layer (2 + 6 l): input norm, Wqkv, Wo, post-attention norm, Wgu
+//               (gate/up interleaved), Wd
+//   ModernBERT  0 tok_embeddings, 1/2 embeddings.norm g/b, 3/4 final_norm g/b; per layer (5 + 8 l): attn_norm g/b,
+//               Wqkv, Wo, mlp_norm g/b, Wi (input/gate interleaved), mlp.Wo
+//   Qwen3       Mistral's, with q_norm, k_norm (fp32 [128]) after the six of each layer (2 + 8 l)
+// Indexed by B2E_ARCH_*.
+constexpr Family kFamilies[] = {
+    {5, 12, 0, 2, 6, 8, false, B2E_EPI_BIAS_GELU, NORM_POST_LN, 10, 11, run_bert_trunk},        // B2E_ARCH_BERT
+    {3, 12, 2, 4, 8, 10, false, B2E_EPI_BIAS_GELU, NORM_ADD_LN, 1, 2, run_esm_trunk},           // B2E_ARCH_ESM2
+    {2, 6, 1, 2, 4, 5, true, B2E_EPI_SWIGLU, NORM_ADD_RMS, 1, -1, run_mistral_trunk},          // B2E_ARCH_MISTRAL
+    {5, 8, 2, 3, 6, 7, true, B2E_EPI_GEGLU, NORM_ADD_LN, 3, 4, run_modernbert_trunk},          // B2E_ARCH_MODERNBERT
+    {2, 8, 1, 2, 4, 5, true, B2E_EPI_SWIGLU, NORM_ADD_RMS, 1, -1, run_mistral_trunk},          // B2E_ARCH_QWEN3
+};
+
+const Family* family(int arch) {
+  return arch >= 0 && arch < (int)(sizeof kFamilies / sizeof kFamilies[0]) ? &kFamilies[arch] : nullptr;
+}
+
+// Rotary cos / sin tables [max_pos, cols] of the families that rotate q and k, built once.  Each table's kernel and
+// arguments decide results bit for bit: ESM-2 at head_dim 64 keeps rope_table_kernel, ESM-2 at head_dim 32 builds
+// angle(p, i) = p * 10000^(-2i/32) over 16 columns, ModernBERT one table per layer type (rope_theta for the
+// full-attention layers, rope_theta_local for the sliding ones), Mistral / Qwen3 64 columns of rope_theta.
+int make_rope_tables(B2EEncoder* e) {
+  const B2EModelDesc& d = e->desc;
+  if (d.arch == B2E_ARCH_BERT) return B2E_OK;
+  const bool esm = d.arch == B2E_ARCH_ESM2, two = d.arch == B2E_ARCH_MODERNBERT;
+  const int cols = is_decoder(d.arch) ? 64 : (esm && d.head_dim == 32) ? 16 : 32;
+  const size_t n = (size_t)d.max_pos * cols;
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  if (cudaMalloc(&e->rope_cos, n * sizeof(float)) != cudaSuccess ||
+      cudaMalloc(&e->rope_sin, n * sizeof(float)) != cudaSuccess ||
+      (two && (cudaMalloc(&e->rope_cos2, n * sizeof(float)) != cudaSuccess ||
+               cudaMalloc(&e->rope_sin2, n * sizeof(float)) != cudaSuccess)))
+    return fail(B2E_ERR_CUDA, "cudaMalloc of the rotary tables failed");
+  if (esm && d.head_dim == 64)
+    rope_table_kernel<<<grid, 256>>>(e->rope_cos, e->rope_sin, d.max_pos);
+  else
+    rope_table_theta_kernel<<<grid, 256>>>(e->rope_cos, e->rope_sin, d.max_pos, cols, esm ? 10000.0f : d.rope_theta);
+  if (two) rope_table_theta_kernel<<<grid, 256>>>(e->rope_cos2, e->rope_sin2, d.max_pos, cols, d.rope_theta_local);
+  if (cudaDeviceSynchronize() != cudaSuccess)
+    return fail(B2E_ERR_CUDA, "rotary table kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
+  return B2E_OK;
+}
+
+// The final norm of b2e_encode over the padded [B*S] rows, into float or the storage type.
+template <typename OutT>
+int launch_final_norm(B2EEncoder* e, int M, OutT* out, cudaStream_t st) {
+  const B2EModelDesc& d = e->desc;
+  const float *g = e->final_norm(0), *b = e->final_norm(1);
+  switch (e->fam->norm) {
+    case NORM_POST_LN:
+      DISPATCH_H(d.hidden, (layernorm_kernel<HW, OutT><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                               e->tmp, e->hidden, g, b, out, M, d.eps)));
+      break;
+    case NORM_ADD_LN:   // emb_layer_norm_after / final_norm over (residual stream + last FFN output)
+      DISPATCH_H(d.hidden, (add_layernorm_kernel<HW, OutT><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                               e->xres, e->tmp, g, b, out, M, d.eps)));
+      break;
+    case NORM_ADD_RMS:   // final RMSNorm over (residual stream + last down_proj output)
+      DISPATCH_H(d.hidden, (add_rmsnorm_kernel<HW, OutT><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                               e->xres, e->tmp, g, out, M, d.eps)));
+      break;
   }
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
@@ -1070,12 +1092,8 @@ int b2e_debug_set_layers(B2EEncoder* e, int n) {
 const char* b2e_last_error(void) { return g_err.c_str(); }
 
 int b2e_num_weights(const B2EModelDesc* desc) {
-  if (!desc) return -1;
-  if (desc->arch == B2E_ARCH_BERT) return 5 + 12 * desc->num_layers;
-  if (desc->arch == B2E_ARCH_ESM2) return 3 + 12 * desc->num_layers;
-  if (is_decoder(desc->arch)) return 2 + decoder_layer_slots(desc->arch) * desc->num_layers;
-  if (desc->arch == B2E_ARCH_MODERNBERT) return 5 + 8 * desc->num_layers;
-  return -1;
+  const Family* f = desc ? family(desc->arch) : nullptr;
+  return f ? f->lead + f->stride * desc->num_layers : -1;
 }
 
 // Everything b2e_encoder_create would reject about the SHAPE of a model, without touching a device or
@@ -1132,11 +1150,11 @@ int b2e_check_model(const B2EModelDesc* desc) {
 }
 
 namespace {
-// Mistral family and Qwen3: head_dim 128, grouped-query heads, SwiGLU MLP, no biases.
-int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_weights, const float* const* absmax,
+// absmax: nullptr (16-bit matrices) or 4 * num_layers NF4 scale pointers (b2e_encoder_create_nf4)
+int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_weights, const float* const* absmax,
                    int device, B2EEncoder** out) {
-  const int L = desc->num_layers, H = desc->hidden, I = desc->intermediate;
-  const int QC = (desc->heads + 2 * desc->kv_heads) * 128, CC = desc->heads * 128;
+  if (!desc || !weights || !out) return fail(B2E_ERR_INVALID, "null argument");
+  *out = nullptr;
   int rc;
   if ((rc = b2e_check_model(desc))) return rc;
   if (n_weights != b2e_num_weights(desc))
@@ -1147,118 +1165,31 @@ int create_mistral(const B2EModelDesc* desc, const void* const* weights, int n_w
   if ((rc = device_info(device, &info))) return rc;
   DeviceGuard guard;
   CUDA_TRY(cudaSetDevice(device));
+
   B2EEncoder* e = new B2EEncoder();
   e->desc = *desc;
+  e->fam = family(desc->arch);   // b2e_check_model accepted the architecture
   e->full_layers = desc->num_layers;
   e->w.assign(weights, weights + n_weights);
   e->device = device;
   e->sms = info.sms;
-  e->tm_wqkv.resize(L); e->tm_wo.resize(L); e->tm_w1.resize(L); e->tm_w2.resize(L);
-  for (int l = 0; l < L; ++l) {
-    const float* const* s = absmax ? absmax + 4 * l : nullptr;
-    if ((rc = make_gemm_w(&e->tm_wqkv[l], e->Mi(l, 1), s ? s[0] : nullptr, QC, H, B2E_EPI_BIAS)) ||
-        (rc = make_gemm_w(&e->tm_wo[l], e->Mi(l, 2), s ? s[1] : nullptr, H, CC, B2E_EPI_BIAS)) ||
-        (rc = make_gemm_w(&e->tm_w1[l], e->Mi(l, 4), s ? s[2] : nullptr, 2 * I, H, B2E_EPI_SWIGLU)) ||
-        (rc = make_gemm_w(&e->tm_w2[l], e->Mi(l, 5), s ? s[3] : nullptr, H, I, B2E_EPI_BIAS))) {
-      delete e;
-      return rc;
-    }
-  }
-  const size_t n = (size_t)desc->max_pos * 64;
-  if (cudaMalloc(&e->rope_cos, n * sizeof(float)) != cudaSuccess ||
-      cudaMalloc(&e->rope_sin, n * sizeof(float)) != cudaSuccess) {
-    b2e_encoder_destroy(e);
-    return fail(B2E_ERR_CUDA, "cudaMalloc of the rotary tables failed");
-  }
-  rope_table_theta_kernel<<<(unsigned)((n + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos,
-                                                                64, desc->rope_theta);
-  if (cudaDeviceSynchronize() != cudaSuccess) {
-    b2e_encoder_destroy(e);
-    return fail(B2E_ERR_CUDA, "rotary table kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-  }
-  *out = e;
-  return B2E_OK;
-}
-}  // namespace
-
-namespace {
-// absmax: nullptr (16-bit matrices) or 4 * num_layers NF4 scale pointers (b2e_encoder_create_nf4)
-int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_weights, const float* const* absmax,
-                   int device, B2EEncoder** out) {
-  if (!desc || !weights || !out) return fail(B2E_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (is_decoder(desc->arch)) return create_mistral(desc, weights, n_weights, absmax, device, out);
-  int rc;
-  if ((rc = b2e_check_model(desc))) return rc;
-  if (n_weights != b2e_num_weights(desc))
-    return fail(B2E_ERR_INVALID, "expected %d weight pointers, got %d", b2e_num_weights(desc),
-                n_weights);
-  for (int i = 0; i < n_weights; ++i)
-    if (!weights[i]) return fail(B2E_ERR_INVALID, "weight pointer %d is null", i);
-  DeviceInfo info;
-  if ((rc = device_info(device, &info))) return rc;
-  DeviceGuard guard;
-  CUDA_TRY(cudaSetDevice(device));
-
-  B2EEncoder* e = new B2EEncoder();
-  e->desc = *desc;
-  e->full_layers = desc->num_layers;
-  e->w.assign(weights, weights + n_weights);
-  e->device = device;
-  e->sms = info.sms;
+  const Family& f = *e->fam;
   const int L = desc->num_layers, H = desc->hidden, I = desc->intermediate;
+  const int QC = e->qkv_cols(), CC = e->ctx_cols();
   e->tm_wqkv.resize(L); e->tm_wo.resize(L); e->tm_w1.resize(L); e->tm_w2.resize(L);
-  const bool esm = desc->arch == B2E_ARCH_ESM2;
-  const bool mbert = desc->arch == B2E_ARCH_MODERNBERT;
-  const int n1 = mbert ? 2 * I : I;   // ModernBERT's Wi holds input and gate rows
   for (int l = 0; l < L; ++l) {
-    const void* wqkv = mbert ? e->Mb(l, 2) : esm ? e->E(l, 2) : e->L(l, 0);
-    const void* wo = mbert ? e->Mb(l, 3) : esm ? e->E(l, 4) : e->L(l, 2);
-    const void* w1 = mbert ? e->Mb(l, 6) : esm ? e->E(l, 8) : e->L(l, 6);
-    const void* w2 = mbert ? e->Mb(l, 7) : esm ? e->E(l, 10) : e->L(l, 8);
     const float* const* s = absmax ? absmax + 4 * l : nullptr;
-    if ((rc = make_gemm_w(&e->tm_wqkv[l], wqkv, s ? s[0] : nullptr, 3 * H, H, B2E_EPI_BIAS)) ||
-        (rc = make_gemm_w(&e->tm_wo[l], wo, s ? s[1] : nullptr, H, H, B2E_EPI_BIAS)) ||
-        (rc = make_gemm_w(&e->tm_w1[l], w1, s ? s[2] : nullptr, n1, H, mbert ? B2E_EPI_GEGLU : B2E_EPI_BIAS_GELU)) ||
-        (rc = make_gemm_w(&e->tm_w2[l], w2, s ? s[3] : nullptr, H, I, B2E_EPI_BIAS))) {
-      delete e;
+    if ((rc = make_gemm_w(&e->tm_wqkv[l], e->slot(l, f.wqkv), s ? s[0] : nullptr, QC, H, B2E_EPI_BIAS)) ||
+        (rc = make_gemm_w(&e->tm_wo[l], e->slot(l, f.wo), s ? s[1] : nullptr, H, CC, B2E_EPI_BIAS)) ||
+        (rc = make_gemm_w(&e->tm_w1[l], e->slot(l, f.w1), s ? s[2] : nullptr, f.w1_gated ? 2 * I : I, H, f.w1_epi)) ||
+        (rc = make_gemm_w(&e->tm_w2[l], e->slot(l, f.w2), s ? s[3] : nullptr, H, I, B2E_EPI_BIAS))) {
+      b2e_encoder_destroy(e);
       return rc;
     }
   }
-  if (mbert) {
-    const size_t n = (size_t)desc->max_pos * 32;
-    if (cudaMalloc(&e->rope_cos, n * sizeof(float)) != cudaSuccess ||
-        cudaMalloc(&e->rope_sin, n * sizeof(float)) != cudaSuccess ||
-        cudaMalloc(&e->rope_cos2, n * sizeof(float)) != cudaSuccess ||
-        cudaMalloc(&e->rope_sin2, n * sizeof(float)) != cudaSuccess) {
-      b2e_encoder_destroy(e);
-      return fail(B2E_ERR_CUDA, "cudaMalloc of the rotary tables failed");
-    }
-    rope_table_theta_kernel<<<(unsigned)((n + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos, 32,
-                                                                  desc->rope_theta);
-    rope_table_theta_kernel<<<(unsigned)((n + 255) / 256), 256>>>(e->rope_cos2, e->rope_sin2, desc->max_pos, 32,
-                                                                  desc->rope_theta_local);
-    if (cudaDeviceSynchronize() != cudaSuccess) {
-      b2e_encoder_destroy(e);
-      return fail(B2E_ERR_CUDA, "rotary table kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-  }
-  if (esm) {
-    const size_t n = (size_t)desc->max_pos * 32;
-    if (cudaMalloc(&e->rope_cos, n * sizeof(float)) != cudaSuccess ||
-        cudaMalloc(&e->rope_sin, n * sizeof(float)) != cudaSuccess) {
-      b2e_encoder_destroy(e);
-      return fail(B2E_ERR_CUDA, "cudaMalloc of the rotary tables failed");
-    }
-    if (desc->head_dim == 32)   // [max_pos, 16]: angle(p, i) = p * 10000^(-2i/32)
-      rope_table_theta_kernel<<<(unsigned)((n / 2 + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos, 16,
-                                                                        10000.0f);
-    else
-      rope_table_kernel<<<(unsigned)((n + 255) / 256), 256>>>(e->rope_cos, e->rope_sin, desc->max_pos);
-    if (cudaDeviceSynchronize() != cudaSuccess) {
-      b2e_encoder_destroy(e);
-      return fail(B2E_ERR_CUDA, "rotary table kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-    }
+  if ((rc = make_rope_tables(e))) {
+    b2e_encoder_destroy(e);
+    return rc;
   }
   *out = e;
   return B2E_OK;
@@ -1288,10 +1219,9 @@ void b2e_encoder_destroy(B2EEncoder* e) {
   if (!e) return;
   DeviceGuard guard;
   cudaSetDevice(e->device);
-  cudaFree(e->hidden); cudaFree(e->qkv); cudaFree(e->ctx); cudaFree(e->tmp); cudaFree(e->ffn);
-  cudaFree(e->stage_in); cudaFree(e->stage_out);
-  cudaFree(e->xres); cudaFree(e->tok_scale); cudaFree(e->rope_cos); cudaFree(e->rope_sin);
-  cudaFree(e->rope_cos2); cudaFree(e->rope_sin2);
+  for (DevBuf<h16>* b : {&e->hidden, &e->qkv, &e->ctx, &e->tmp, &e->ffn}) b->release();
+  e->xres.release(); e->tok_scale.release(); e->stage_in.release(); e->stage_out.release();
+  cudaFree(e->rope_cos); cudaFree(e->rope_sin); cudaFree(e->rope_cos2); cudaFree(e->rope_sin2);
   e->pack.release();
   e->drop_graphs();
   e->pool.release();
@@ -1319,49 +1249,9 @@ int b2e_encode(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int
     return fail(B2E_ERR_INVALID, "encode: out_dtype must be F32 or this build's storage type (%d)", kStorageDtype);
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = ensure_workspace(e, B, S))) return rc;
-  const B2EModelDesc& d = e->desc;
-  const int M = B * S, H = d.hidden, l = d.num_layers - 1;
-  if (is_decoder(d.arch)) {
-    if ((rc = run_mistral_trunk(e, ids, mask, B, S, st))) return rc;
-    // final RMSNorm over (residual stream + last down_proj output)
-    if (out_dtype == B2E_DTYPE_F32) {
-      DISPATCH_H(H, (add_rmsnorm_kernel<HW, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, (const float*)e->w[1], (float*)out_hidden, M, d.eps)));
-    } else {
-      DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, (const float*)e->w[1], (h16*)out_hidden, M, d.eps)));
-    }
-    CUDA_TRY(cudaGetLastError());
-    return B2E_OK;
-  }
-  if (d.arch == B2E_ARCH_ESM2 || d.arch == B2E_ARCH_MODERNBERT) {
-    const bool mb = d.arch == B2E_ARCH_MODERNBERT;
-    if ((rc = mb ? run_modernbert_trunk(e, ids, mask, B, S, st) : run_esm_trunk(e, ids, mask, B, S, st))) return rc;
-    // emb_layer_norm_after / final_norm over (residual stream + last FFN output)
-    const float* fg = (const float*)e->w[mb ? 3 : 1];
-    const float* fb = (const float*)e->w[mb ? 4 : 2];
-    if (out_dtype == B2E_DTYPE_F32) {
-      DISPATCH_H(H, (add_layernorm_kernel<HW, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, fg, fb, (float*)out_hidden, M, d.eps)));
-    } else {
-      DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, fg, fb, (h16*)out_hidden, M, d.eps)));
-    }
-    CUDA_TRY(cudaGetLastError());
-    return B2E_OK;
-  }
-  if ((rc = run_bert_trunk(e, ids, mask, types, B, S, st))) return rc;
-  if (out_dtype == B2E_DTYPE_F32) {
-    DISPATCH_H(H, (layernorm_kernel<HW, float><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                       e->tmp, e->hidden, (const float*)e->L(l, 10), (const float*)e->L(l, 11),
-                       (float*)out_hidden, M, d.eps)));
-  } else {
-    DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                       e->tmp, e->hidden, (const float*)e->L(l, 10), (const float*)e->L(l, 11),
-                       (h16*)out_hidden, M, d.eps)));
-  }
-  CUDA_TRY(cudaGetLastError());
-  return B2E_OK;
+  if ((rc = e->fam->trunk(e, ids, mask, types, B, S, st, SeqLayout()))) return rc;
+  if (out_dtype == B2E_DTYPE_F32) return launch_final_norm(e, B * S, (float*)out_hidden, st);
+  return launch_final_norm(e, B * S, (h16*)out_hidden, st);
 }
 
 int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t* types,
@@ -1374,80 +1264,58 @@ int b2e_encode_pooled(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = ensure_workspace(e, B, S))) return rc;
   const B2EModelDesc& d = e->desc;
-  const int H = d.hidden, l = d.num_layers - 1;
+  const int H = d.hidden;
   PoolScratch& ps = e->pool;
   // Pooled paths run on the padding-free token layout (pack.cuh): only attended tokens go through the GEMMs, norms
   // and attention query tiles; nothing here can observe a padded position.
   SeqLayout lay;
   if ((rc = pack_prepare(e->pack, mask, B, S, packing_enabled(), st, &lay))) return rc;
-  if (is_decoder(d.arch)) {
-    if ((rc = run_mistral_trunk(e, ids, mask, B, S, st, lay))) return rc;
-    if (pool_kind == B2E_POOL_LAST_TOKEN) {
-      // only the B selected rows go through the final norm (fp32 end to end)
-      seq_len_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, ps.seq_len, B, S);
-      last_token_index_kernel<<<1, 256, 0, st>>>(mask, ps.seq_len, ps.idx, B, S);
-      DISPATCH_H(H, (rmsnorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, (const float*)e->w[1], ps.idx, out, B, S, d.eps, lay.cu)));
-      if (l2) l2_normalize_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B, H);
-      CUDA_TRY(cudaGetLastError());
-      return B2E_OK;
-    }
-    // mean poolers: final RMSNorm fused with the masked sum, fp32 end to end, [B,S,H] never written
-    if ((rc = launch_pool_weights(ps, const_cast<int64_t*>(mask), B, S, pool_kind, 0, st))) return rc;
-    const int nsplit = pool_nsplit(S);
-    const int rows_per = (S + nsplit - 1) / nsplit;
-    dim3 grid(B, nsplit);
-    DISPATCH_H(H, (addnorm_pool_kernel<HW, true><<<grid, ROW_THREADS, 0, st>>>(
-                       e->xres, e->tmp, (const float*)e->w[1], nullptr, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
-    CUDA_TRY(cudaGetLastError());
-    return launch_finalize(ps, out, B, H, nsplit, l2, /*round_mode=*/0, st);
-  }
-  if (d.arch == B2E_ARCH_ESM2 || d.arch == B2E_ARCH_MODERNBERT) {
-    const bool mb = d.arch == B2E_ARCH_MODERNBERT;
-    if ((rc = mb ? run_modernbert_trunk(e, ids, mask, B, S, st, lay) : run_esm_trunk(e, ids, mask, B, S, st, lay)))
-      return rc;
-    const float* fg = (const float*)e->w[mb ? 3 : 1];
-    const float* fb = (const float*)e->w[mb ? 4 : 2];
-    if (pool_kind == B2E_POOL_LAST_TOKEN) {
-      // only the B selected rows go through emb_layer_norm_after (fp32 end to end)
-      seq_len_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, ps.seq_len, B, S);
-      last_token_index_kernel<<<1, 256, 0, st>>>(mask, ps.seq_len, ps.idx, B, S);
-      DISPATCH_H(H, (addnorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
-                         e->xres, e->tmp, fg, fb, ps.idx, out, B, S, d.eps, lay.cu)));
-      if (l2) l2_normalize_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B, H);
-      CUDA_TRY(cudaGetLastError());
-      return B2E_OK;
-    }
-    // mean poolers: final LayerNorm fused with the masked sum, fp32 end to end, [B,S,H] never written
-    if ((rc = launch_pool_weights(ps, const_cast<int64_t*>(mask), B, S, pool_kind, 0, st))) return rc;
-    const int nsplit = pool_nsplit(S);
-    const int rows_per = (S + nsplit - 1) / nsplit;
-    dim3 grid(B, nsplit);
-    DISPATCH_H(H, (addnorm_pool_kernel<HW, false><<<grid, ROW_THREADS, 0, st>>>(
-                       e->xres, e->tmp, fg, fb, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
-    CUDA_TRY(cudaGetLastError());
-    return launch_finalize(ps, out, B, H, nsplit, l2, /*round_mode=*/0, st);
-  }
-  if ((rc = run_bert_trunk(e, ids, mask, types, B, S, st, lay))) return rc;
-  const float* g = (const float*)e->L(l, 10);
-  const float* bt = (const float*)e->L(l, 11);
+  if ((rc = e->fam->trunk(e, ids, mask, types, B, S, st, lay))) return rc;
+  const FinalNorm norm = e->fam->norm;
+  const float *g = e->final_norm(0), *bt = e->final_norm(1);
   if (pool_kind == B2E_POOL_LAST_TOKEN) {
+    // only the B selected rows go through the final norm (fp32 end to end)
     seq_len_kernel<<<(B + 7) / 8, 256, 0, st>>>(mask, ps.seq_len, B, S);
     last_token_index_kernel<<<1, 256, 0, st>>>(mask, ps.seq_len, ps.idx, B, S);
-    DISPATCH_H(H, (layernorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
-                       e->tmp, e->hidden, ps.idx, g, bt, out, B, S, d.eps, lay.cu)));
+    switch (norm) {
+      case NORM_POST_LN:
+        DISPATCH_H(H, (layernorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
+                           e->tmp, e->hidden, ps.idx, g, bt, out, B, S, d.eps, lay.cu)));
+        break;
+      case NORM_ADD_LN:
+        DISPATCH_H(H, (addnorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
+                           e->xres, e->tmp, g, bt, ps.idx, out, B, S, d.eps, lay.cu)));
+        break;
+      case NORM_ADD_RMS:
+        DISPATCH_H(H, (rmsnorm_gather_kernel<HW><<<row_blocks(B), ROW_THREADS, 0, st>>>(
+                           e->xres, e->tmp, g, ps.idx, out, B, S, d.eps, lay.cu)));
+        break;
+    }
     if (l2) l2_normalize_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B, H);
     CUDA_TRY(cudaGetLastError());
     return B2E_OK;
   }
-  // the fused path never edits the caller's mask: weights are built from a read-only view
+  // mean poolers: the final norm fused with the masked sum, fp32 end to end, [B,S,H] never written.  The fused path
+  // never edits the caller's mask: weights are built from a read-only view.
   if ((rc = launch_pool_weights(ps, const_cast<int64_t*>(mask), B, S, pool_kind, /*mutate=*/0, st)))
     return rc;
   const int nsplit = pool_nsplit(S);
   const int rows_per = (S + nsplit - 1) / nsplit;
   dim3 grid(B, nsplit);
-  DISPATCH_H(H, (layernorm_pool_kernel<HW><<<grid, ROW_THREADS, 0, st>>>(
-                     e->tmp, e->hidden, g, bt, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
+  switch (norm) {
+    case NORM_POST_LN:
+      DISPATCH_H(H, (layernorm_pool_kernel<HW><<<grid, ROW_THREADS, 0, st>>>(
+                         e->tmp, e->hidden, g, bt, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
+      break;
+    case NORM_ADD_LN:
+      DISPATCH_H(H, (addnorm_pool_kernel<HW, false><<<grid, ROW_THREADS, 0, st>>>(
+                         e->xres, e->tmp, g, bt, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
+      break;
+    case NORM_ADD_RMS:
+      DISPATCH_H(H, (addnorm_pool_kernel<HW, true><<<grid, ROW_THREADS, 0, st>>>(
+                         e->xres, e->tmp, g, bt, ps.w, ps.part, S, rows_per, d.eps, lay.cu)));
+      break;
+  }
   CUDA_TRY(cudaGetLastError());
   return launch_finalize(ps, out, B, H, nsplit, l2, /*round_mode=*/0, st);
 }
@@ -1467,23 +1335,8 @@ int b2e_embed_host(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
   const int H = e->desc.hidden;
   // two input slots (ids | mask | types) so batch i+1 uploads while batch i computes
   const size_t slot = (size_t)batch * S * 3;
-  if (2 * slot > e->stage_cap) {
-    ++e->ws_gen;
-    cudaFree(e->stage_in);
-    e->stage_in = nullptr;
-    e->stage_cap = 0;
-    CUDA_TRY(cudaMalloc(&e->stage_in, 2 * slot * sizeof(int64_t)));
-    e->stage_cap = 2 * slot;
-  }
-  const size_t out_elems = (size_t)batch * H * 2;
-  if (out_elems > e->stage_out_cap) {
-    ++e->ws_gen;
-    cudaFree(e->stage_out);
-    e->stage_out = nullptr;
-    e->stage_out_cap = 0;
-    CUDA_TRY(cudaMalloc(&e->stage_out, out_elems * sizeof(float)));
-    e->stage_out_cap = out_elems;
-  }
+  if ((rc = e->stage_in.grow(2 * slot, e->ws_gen)) || (rc = e->stage_out.grow((size_t)batch * H * 2, e->ws_gen)))
+    return rc;
   static const bool use_graphs = [] {
     const char* v = getenv("B2E_GRAPHS");   // B2E_GRAPHS=0: every batch launches its kernels one by one
     return !(v && v[0] == '0');
@@ -1797,27 +1650,17 @@ int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, 
 // ---- exact inner-product top-k (retrieval query path)
 extern "C++" {
 namespace {
-struct TopkScratch {
-  float* score = nullptr;
-  int64_t* index = nullptr;
-  size_t cap = 0;
-  int device = -1;
+struct TopkScratch : DeviceScratch {
+  DevBuf<float> score;
+  DevBuf<int64_t> index;
   int ensure(size_t elems) {
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (dev != device) {
-      cudaFree(score); cudaFree(index);
-      score = nullptr; index = nullptr; cap = 0;
-      device = dev;
-    }
-    if (elems > cap) {
-      cudaFree(score); cudaFree(index);
-      score = nullptr; index = nullptr; cap = 0;
-      CUDA_TRY(cudaMalloc(&score, elems * sizeof(float)));
-      CUDA_TRY(cudaMalloc(&index, elems * sizeof(int64_t)));
-      cap = elems;
-    }
+    int rc;
+    if ((rc = follow_device(*this)) || (rc = score.grow(elems, gen)) || (rc = index.grow(elems, gen))) return rc;
     return B2E_OK;
+  }
+  void release() {
+    score.release();
+    index.release();
   }
 };
 thread_local TopkScratch g_topk_scratch;
@@ -1861,45 +1704,27 @@ int launch_topk(const float* queries, int Q, const T* corpus, int64_t N, int H, 
 }
 
 // ---- tensor-core fast path (topk_tc.cuh)
-struct TcScratch {
-  float* scores = nullptr;      // [tiles * 128, 16]
-  float* qpad = nullptr;        // [16, H]
-  TcQuery* meta = nullptr;      // [16]
-  unsigned* hist = nullptr;     // [16, TC_BINS]
-  unsigned* cand = nullptr;     // [16, TC_MAX_CAND]
-  unsigned* n_cand = nullptr;   // [16]
-  int* flag = nullptr;          // [2]: fallback requested; passes that requested it (debug)
-  float* norm2 = nullptr;       // [1]
-  size_t cap_rows = 0, cap_h = 0;
-  int device = -1;
-  void release() {
-    cudaFree(scores); cudaFree(qpad); cudaFree(meta); cudaFree(hist); cudaFree(cand); cudaFree(n_cand);
-    cudaFree(flag); cudaFree(norm2);
-    scores = qpad = norm2 = nullptr; meta = nullptr; hist = cand = n_cand = nullptr; flag = nullptr;
-    cap_rows = cap_h = 0;
-  }
+struct TcScratch : DeviceScratch {
+  DevBuf<float> scores;       // [tiles * 128, 16]
+  DevBuf<float> qpad;         // [16, H]
+  DevBuf<TcQuery> meta;       // [16]
+  DevBuf<unsigned> hist;      // [16, TC_BINS]
+  DevBuf<unsigned> cand;      // [16, TC_MAX_CAND]
+  DevBuf<unsigned> n_cand;    // [16]
+  DevBuf<int> flag;           // [2]: fallback requested; passes that requested it (debug); zeroed on allocation
+  DevBuf<float> norm2;        // [1]
   int ensure(size_t rows, size_t h) {
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (dev != device) {
-      release();
-      device = dev;
-    }
-    if (rows <= cap_rows && h <= cap_h && flag != nullptr) return B2E_OK;
-    const size_t r = rows > cap_rows ? rows : cap_rows, hh = h > cap_h ? h : cap_h;
-    release();
-    CUDA_TRY(cudaMalloc(&scores, r * TC_NQ * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&qpad, (size_t)TC_NQ * hh * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&meta, TC_NQ * sizeof(TcQuery)));
-    CUDA_TRY(cudaMalloc(&hist, (size_t)TC_NQ * TC_BINS * sizeof(unsigned)));
-    CUDA_TRY(cudaMalloc(&cand, (size_t)TC_NQ * TC_MAX_CAND * sizeof(unsigned)));
-    CUDA_TRY(cudaMalloc(&n_cand, TC_NQ * sizeof(unsigned)));
-    CUDA_TRY(cudaMalloc(&flag, 2 * sizeof(int)));
-    CUDA_TRY(cudaMalloc(&norm2, sizeof(float)));
-    CUDA_TRY(cudaMemset(flag, 0, 2 * sizeof(int)));
-    cap_rows = r;
-    cap_h = hh;
+    int rc;
+    if ((rc = follow_device(*this)) || (rc = scores.grow(rows * TC_NQ, gen)) || (rc = qpad.grow(TC_NQ * h, gen)) ||
+        (rc = meta.grow(TC_NQ, gen)) || (rc = hist.grow((size_t)TC_NQ * TC_BINS, gen)) ||
+        (rc = cand.grow((size_t)TC_NQ * TC_MAX_CAND, gen)) || (rc = n_cand.grow(TC_NQ, gen)) ||
+        (rc = flag.grow(2, gen, true)) || (rc = norm2.grow(1, gen)))
+      return rc;
     return B2E_OK;
+  }
+  void release() {
+    scores.release(); qpad.release(); meta.release(); hist.release(); cand.release(); n_cand.release();
+    flag.release(); norm2.release();
   }
 };
 thread_local TcScratch g_tc_scratch;
@@ -1995,7 +1820,7 @@ int b2e_topk_ip_tc(const float* queries, int Q, const float* corpus, int64_t N, 
 int b2e_debug_topk_tc_fell_back(int* out) {
   if (!out) return fail(B2E_ERR_INVALID, "null pointer");
   *out = 0;
-  if (g_tc_scratch.flag == nullptr) return B2E_OK;
+  if (g_tc_scratch.flag.p == nullptr) return B2E_OK;
   CUDA_TRY(cudaDeviceSynchronize());
   CUDA_TRY(cudaMemcpy(out, g_tc_scratch.flag, sizeof(int), cudaMemcpyDeviceToHost));
   return B2E_OK;
@@ -2004,37 +1829,23 @@ int b2e_debug_topk_tc_fell_back(int* out) {
 // ---- ubinary retrieval: packed bits, Hamming top-K, float rescoring (binsearch.cuh)
 extern "C++" {
 namespace {
-struct BinScratch {
-  uint32_t* qbits = nullptr;            // [Q, W]
-  unsigned* hist = nullptr;             // [Q, H+1]
-  int* thr = nullptr;                   // [Q, 2]
-  unsigned long long* cand = nullptr;   // [Q, BIN_MAX_CAND]
-  unsigned* n_cand = nullptr;           // [Q]
-  size_t cap_q = 0, cap_h = 0;
-  int device = -1;
-  void release() {
-    cudaFree(qbits); cudaFree(hist); cudaFree(thr); cudaFree(cand); cudaFree(n_cand);
-    qbits = nullptr; hist = nullptr; thr = nullptr; cand = nullptr; n_cand = nullptr;
-    cap_q = cap_h = 0;
-  }
+struct BinScratch : DeviceScratch {
+  DevBuf<uint32_t> qbits;               // [Q, W]
+  DevBuf<unsigned> hist;                // [Q, H+1]
+  DevBuf<int> thr;                      // [Q, 2]
+  DevBuf<unsigned long long> cand;      // [Q, BIN_MAX_CAND]
+  DevBuf<unsigned> n_cand;              // [Q]
   int ensure(int Q, int H) {
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (dev != device) {
-      release();
-      device = dev;
-    }
-    if ((size_t)Q <= cap_q && (size_t)H <= cap_h) return B2E_OK;
-    release();
+    // sized for at least 8 queries of 1024 columns
     const size_t q = (size_t)Q > 8 ? Q : 8, h = (size_t)H > 1024 ? H : 1024;
-    CUDA_TRY(cudaMalloc(&qbits, q * (h / 32) * sizeof(uint32_t)));
-    CUDA_TRY(cudaMalloc(&hist, q * (h + 1) * sizeof(unsigned)));
-    CUDA_TRY(cudaMalloc(&thr, q * 2 * sizeof(int)));
-    CUDA_TRY(cudaMalloc(&cand, q * BIN_MAX_CAND * sizeof(unsigned long long)));
-    CUDA_TRY(cudaMalloc(&n_cand, q * sizeof(unsigned)));
-    cap_q = q;
-    cap_h = h;
+    int rc;
+    if ((rc = follow_device(*this)) || (rc = qbits.grow(q * (h / 32), gen)) || (rc = hist.grow(q * (h + 1), gen)) ||
+        (rc = thr.grow(q * 2, gen)) || (rc = cand.grow(q * BIN_MAX_CAND, gen)) || (rc = n_cand.grow(q, gen)))
+      return rc;
     return B2E_OK;
+  }
+  void release() {
+    qbits.release(); hist.release(); thr.release(); cand.release(); n_cand.release();
   }
 };
 thread_local BinScratch g_bin_scratch;
@@ -2097,7 +1908,7 @@ int b2e_search_ubinary(const float* queries, int Q, const uint8_t* corpus_bits, 
   if ((rc = sc.ensure(Q, H))) return rc;
   const int W = H / 32;
   const uint32_t* corpus = reinterpret_cast<const uint32_t*>(corpus_bits);
-  if ((rc = b2e_pack_ubinary(queries, Q, H, reinterpret_cast<uint8_t*>(sc.qbits), stream))) return rc;
+  if ((rc = b2e_pack_ubinary(queries, Q, H, reinterpret_cast<uint8_t*>(sc.qbits.p), stream))) return rc;
   CUDA_TRY(cudaMemsetAsync(sc.hist, 0, (size_t)Q * (H + 1) * sizeof(unsigned), st));
   CUDA_TRY(cudaMemsetAsync(sc.n_cand, 0, (size_t)Q * sizeof(unsigned), st));
   long long want = (N + BIN_THREADS - 1) / BIN_THREADS;
