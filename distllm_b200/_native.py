@@ -92,6 +92,7 @@ DEBUG_EXPORTS = (
     'b2e_debug_set_packing',
     'b2e_debug_set_gemm_bn',
     'b2e_debug_gemm_bn',
+    'b2e_debug_gemm_rows',
     'b2e_debug_topk_tc_fell_back',
     'b2e_debug_attention_packed',
 )
@@ -252,10 +253,14 @@ def gemm_h16(
     epilogue: int = EPI_BIAS,
 ) -> torch.Tensor:
     """out[M,N] = epi(a[M,K] @ w[N,K].T + bias (+ resid)) on the wgmma GEMM; float16 or bfloat16 in/out (the
-    matching build of the library is used), fp32 accumulation.
+    matching build of the library is used), fp32 accumulation.  ``EPI_BIAS_RESID`` sums ``acc + bias + resid``
+    in fp32; the result is rounded to nearest-even once, and in float16 values beyond +-65504 saturate to
+    +-65504 instead of becoming inf.
 
     ``EPI_SWIGLU``: ``w`` holds gate/up rows interleaved in blocks of 64 (weights.interleave_gate_up)
-    and the result is ``silu(gate) * up`` of shape [M, N/2]."""
+    and the result is ``silu(gate) * up`` of shape [M, N/2]; ``EPI_GEGLU`` the same with erf-GELU.  The gated
+    epilogues take no ``bias``, and only ``EPI_BIAS_RESID`` takes ``resid``: passing one anyway raises
+    ``NativeError`` rather than dropping it."""
     if a.dtype != w.dtype:
         raise NativeError(f'gemm_h16: operands differ in dtype ({a.dtype} vs {w.dtype})')
     lib = load(storage_of(a.dtype))
@@ -281,7 +286,8 @@ def gemm_nf4(
     epilogue: int = EPI_BIAS,
 ) -> torch.Tensor:
     """:func:`gemm_h16` with W in NF4 (embed/encoders/nf4.py: nf4_quantize): ``codes`` uint8 [N, K/2] and
-    ``absmax`` fp32 [K/64, N].  Equals bit for bit ``gemm_h16`` on the dequantised W in ``a``'s storage type."""
+    ``absmax`` fp32 [K/64, N].  Equals bit for bit ``gemm_h16`` on the dequantised W in ``a``'s storage type,
+    with the same rules for ``bias`` and ``resid``."""
     lib = load(storage_of(a.dtype))
     _cuda_contig(a, 'a'), _cuda_contig(codes, 'codes'), _cuda_contig(absmax, 'absmax')
     if bias is not None:

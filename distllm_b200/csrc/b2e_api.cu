@@ -1511,39 +1511,48 @@ int b2e_adjacent_cosine_dist(const void* emb, int dtype, int64_t n_rows, int H,
   return B2E_OK;
 }
 
-int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* resid, void* out,
-                  int M, int N, int K, int epi, void* stream) {
+extern "C++" {
+namespace {
+// b2e_gemm_h16 (absmax null), b2e_gemm_nf4 and b2e_debug_gemm_rows (m_dev set).  An argument the epilogue would not
+// read is an error rather than silently dropped: the gated epilogues add no bias, only B2E_EPI_BIAS_RESID adds resid.
+int gemm_entry(const void* A, const void* W, const float* absmax, const float* bias, const void* resid, void* out,
+               int M, int N, int K, int epi, const int* m_dev, void* stream) {
   if (!A || !W || !out) return fail(B2E_ERR_INVALID, "null tensor pointer");  // bias may be null
+  if (absmax && reinterpret_cast<uintptr_t>(absmax) % 16 != 0)
+    return fail(B2E_ERR_INVALID, "absmax not 16-byte aligned");
   if (epi == B2E_EPI_BIAS_RESID && !resid) return fail(B2E_ERR_INVALID, "resid epilogue needs resid");
+  if (epi != B2E_EPI_BIAS_RESID && resid) return fail(B2E_ERR_INVALID, "gemm: epilogue %d reads no resid", epi);
+  if (epi_is_glu(epi) && bias) return fail(B2E_ERR_INVALID, "gemm: the gated epilogues add no bias");
   int rc;
   if ((rc = check_gemm_shape(M, N, K))) return rc;
-  if ((epi == B2E_EPI_SWIGLU || epi == B2E_EPI_GEGLU) && N % 256 != 0)
+  if (epi_is_glu(epi) && N % 256 != 0)
     return fail(B2E_ERR_INVALID, "gemm: the gated epilogues need N %% 256 == 0 (got %d)", N);
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   CUtensorMap ta;
   GemmW tb;
   if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
-  if ((rc = make_gemm_w(&tb, W, nullptr, N, K, epi))) return rc;
-  return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
+  if ((rc = make_gemm_w(&tb, W, absmax, N, K, epi))) return rc;
+  return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream, m_dev);
+}
+}  // namespace
+}  // extern "C++"
+
+int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* resid, void* out,
+                  int M, int N, int K, int epi, void* stream) {
+  return gemm_entry(A, W, nullptr, bias, resid, out, M, N, K, epi, nullptr, stream);
 }
 
 int b2e_gemm_nf4(const void* A, const void* codes, const float* absmax, const float* bias, const void* resid,
                  void* out, int M, int N, int K, int epi, void* stream) {
-  if (!A || !codes || !absmax || !out) return fail(B2E_ERR_INVALID, "null tensor pointer");  // bias may be null
-  if (reinterpret_cast<uintptr_t>(absmax) % 16 != 0) return fail(B2E_ERR_INVALID, "absmax not 16-byte aligned");
-  if (epi == B2E_EPI_BIAS_RESID && !resid) return fail(B2E_ERR_INVALID, "resid epilogue needs resid");
-  int rc;
-  if ((rc = check_gemm_shape(M, N, K))) return rc;
-  if ((epi == B2E_EPI_SWIGLU || epi == B2E_EPI_GEGLU) && N % 256 != 0)
-    return fail(B2E_ERR_INVALID, "gemm: the gated epilogues need N %% 256 == 0 (got %d)", N);
-  DeviceInfo info;
-  if ((rc = current_device_info(&info))) return rc;
-  CUtensorMap ta;
-  GemmW tb;
-  if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
-  if ((rc = make_gemm_w(&tb, codes, absmax, N, K, epi))) return rc;
-  return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream);
+  if (!absmax) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  return gemm_entry(A, codes, absmax, bias, resid, out, M, N, K, epi, nullptr, stream);
+}
+
+int b2e_debug_gemm_rows(const void* A, const void* W, const float* absmax, const float* bias, const void* resid,
+                        void* out, int M, int N, int K, int epi, const int* m_dev, void* stream) {
+  if (!m_dev) return fail(B2E_ERR_INVALID, "null m_dev");
+  return gemm_entry(A, W, absmax, bias, resid, out, M, N, K, epi, m_dev, stream);
 }
 
 int b2e_attention_d64(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,

@@ -54,11 +54,13 @@ enum {
   B2E_POOL_LAST_TOKEN = 2
 };
 enum {
-  B2E_EPI_BIAS = 0,
-  B2E_EPI_BIAS_GELU = 1,
-  B2E_EPI_BIAS_RESID = 2,
-  B2E_EPI_SWIGLU = 3, /* W rows = gate/up interleaved in blocks of 64; out = silu(gate)*up [M, N/2]; no bias */
-  B2E_EPI_GEGLU = 4   /* same layout, out = gelu(first half) * second half (ModernBERT's Wi: input | gate) */
+  B2E_EPI_BIAS = 0,       /* acc (+ bias); resid must be NULL */
+  B2E_EPI_BIAS_GELU = 1,  /* erf-GELU(acc (+ bias)); resid must be NULL */
+  B2E_EPI_BIAS_RESID = 2, /* acc (+ bias) + resid, summed in fp32 and rounded once; resid required */
+  B2E_EPI_SWIGLU = 3, /* W rows = gate/up interleaved in blocks of 64; out = silu(gate)*up [M, N/2]; bias and
+                         resid must be NULL */
+  B2E_EPI_GEGLU = 4   /* same layout, out = gelu(first half) * second half (ModernBERT's Wi: input | gate); bias
+                         and resid must be NULL */
 };
 
 typedef struct B2EModelDesc {
@@ -163,7 +165,9 @@ int b2e_l2_normalize(float* x, int64_t n_rows, int H, void* stream);
 int b2e_adjacent_cosine_dist(const void* emb, int dtype, int64_t n_rows, int H,
                              const int32_t* doc_id, float* out, void* stream);
 
-/* Building blocks (storage type, row-major, fp32 accumulation): out[M,N] = epi(A[M,K] . W[N,K]^T + bias [+ resid]). */
+/* Building blocks (storage type, row-major, fp32 accumulation): out[M,N] = epi(A[M,K] . W[N,K]^T + bias [+ resid]).
+ * The fp32 result is rounded to nearest-even once; in the half build values beyond +-65504 saturate to +-65504
+ * (bfloat16 has fp32's range).  A bias or resid the epilogue does not read (see B2E_EPI_*) is B2E_ERR_INVALID. */
 int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* resid, void* out,
                   int M, int N, int K, int epilogue, void* stream);
 /* The same with W in NF4: codes uint8 [N, K/2] and fp32 scales absmax [K/64, N] (see b2e_encoder_create_nf4). */

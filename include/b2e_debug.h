@@ -33,6 +33,11 @@ int b2e_debug_set_clock_buffer(void* device_buffer);
 int b2e_debug_set_gemm_bn(int bn);
 /* *out = the tile width a W map of n rows for epilogue epi (B2E_EPI_*) gets now, NF4 (nf4 != 0) or 16-bit */
 int b2e_debug_gemm_bn(int n, int epi, int nf4, int* out);
+/* b2e_gemm_h16 (absmax NULL) or b2e_gemm_nf4 (W = codes, absmax set) with the row count the encoders' packed
+ * forward passes use: *m_dev (device int, 0 <= *m_dev <= M) rows are computed, the rows from *m_dev to M are not
+ * written.  M sizes the grid and the tensor maps. */
+int b2e_debug_gemm_rows(const void* A, const void* W, const float* absmax, const float* bias, const void* resid,
+                        void* out, int M, int N, int K, int epi, const int* m_dev, void* stream);
 /* 0: keep the padded [B, S] token layout on every path; 1 (default, also B2E_PACKED=1): pooled forward passes run
  * on the attended tokens only (csrc/pack.cuh).  Drops the handle's cached CUDA graphs' validity: call it before
  * b2e_embed_host, not between its batches. */

@@ -104,6 +104,24 @@ def test_argument_validation_without_touching_the_gpu():
     assert lib.b2e_encode(None, None, None, None, 1, 1, None, 0, None) == 1
 
 
+@pytest.mark.skipif(torch.cuda.is_available(), reason='placeholder pointers: CPU-only (the GPU suite uses tensors)')
+def test_gemm_rejects_a_bias_or_resid_its_epilogue_does_not_read():
+    """Checked before the device is touched: a gated epilogue adds no bias, only B2E_EPI_BIAS_RESID adds resid."""
+    fake = C.c_void_p(1 << 20)   # never dereferenced: the arguments are rejected first
+    for lib in (_native.load('f16'), _native.load('bf16')):
+        for epi in (_native.EPI_SWIGLU, _native.EPI_GEGLU):
+            assert lib.b2e_gemm_h16(fake, fake, fake, None, fake, 128, 256, 64, epi, None) == 1
+            assert b'no bias' in lib.b2e_last_error()
+            assert lib.b2e_gemm_nf4(fake, fake, fake, fake, None, fake, 128, 256, 64, epi, None) == 1
+            assert b'no bias' in lib.b2e_last_error()
+        for epi in (_native.EPI_BIAS, _native.EPI_BIAS_GELU, _native.EPI_SWIGLU, _native.EPI_GEGLU):
+            assert lib.b2e_gemm_h16(fake, fake, None, fake, fake, 128, 256, 64, epi, None) == 1
+            assert b'reads no resid' in lib.b2e_last_error()
+        # accepted combinations get as far as the device check
+        assert lib.b2e_gemm_h16(fake, fake, fake, fake, fake, 128, 256, 64, _native.EPI_BIAS_RESID, None) == 4
+        assert lib.b2e_gemm_h16(fake, fake, None, None, fake, 128, 256, 64, _native.EPI_SWIGLU, None) == 4
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason='CPU-only behaviour')
 def test_no_cpu_fallback():
     x = torch.zeros(4, 256)
