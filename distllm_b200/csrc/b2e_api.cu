@@ -195,7 +195,7 @@ int check_gemm_shape(int M, int N, int K) {
   return B2E_OK;
 }
 
-bool g_gemm_profiling = false;   // b2e_debug_set_clock_buffer: the bias GEMM runs its timeline instantiation
+bool g_gemm_profiling = false;   // b2e_debug_set_clock_buffer: the bias and bias + GELU GEMMs run their timeline instantiations
 
 // B2E_GEMM_BN=128 | 192 or b2e_debug_set_gemm_bn forces the GEMM tile width of the W maps built from then on (A/B
 // measurements, the equality tests); 0: the rule of gemm_bn
@@ -238,7 +238,7 @@ template <int EPI>
 int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const float* bias,
                     const h16* resid, int M, int N, int K, cudaStream_t st, const int* m_dev) {
   auto kern = gemm_h16_wgmma_kernel<EPI>;
-  int smem = GEMM_SMEM_BYTES;
+  int smem = GemmPlan<false>::SMEM_BYTES;
   if (N % wb.bn != 0) return fail(B2E_ERR_INVALID, "gemm: N=%d is not a multiple of its W map's tile width %d", N, wb.bn);
   if (wb.absmax) {
     kern = gemm_h16_wgmma_kernel<EPI, false, true>;
@@ -249,10 +249,10 @@ int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const flo
     } else {
       kern = gemm_h16_wgmma_kernel<EPI, false, false, 192>;
       smem = GemmPlan<false, 192>::SMEM_BYTES;
-      if constexpr (EPI == EPI_BIAS)
+      if constexpr (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU)
         if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true, false, 192>;
     }
-  } else if constexpr (EPI == EPI_BIAS) {
+  } else if constexpr (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU) {
     if (g_gemm_profiling) kern = gemm_h16_wgmma_kernel<EPI, true>;
   }
   int rc = ensure_smem_attr(kern, smem);

@@ -8,6 +8,13 @@
 //                 epilogue (+bias, erf-GELU | +residual | gated activation) runs on those registers, writes h16
 //                 pairs into the warpgroup's swizzled staging tile and one thread stores it with TMA
 //
+// The epilogue picks its path once per tile.  A tile inside the device rows runs straight-line code: the tile's
+// bias comes from the consumer's slot in shared memory (loaded from global memory when the turn starts, written
+// after the main loop), two 8-column groups of both 64-row halves per step (16 independent pairs, so the GELU
+// chains overlap), and each group pair goes into the staging tile with one stmatrix.x4 per half -- no row test,
+// no global address and no branch inside the element loop.  The last row tile crossing M stores its rows from
+// registers, one row test per pair.
+//
 // BN (the tile width) is 128 or 192 (GemmPlan).  A 192-wide tile moves a sixth fewer operand bytes through L2 and
 // shared memory per FLOP than a 128-wide one; each output element sums the same products in the same order at
 // either width, so both give the same bits.  The NF4 producer (one W row per thread of 128) and the gated
@@ -49,10 +56,6 @@ constexpr int GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;   // 128 x 40 +
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;
 constexpr int GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_BN * GEMM_BK * 2;
 constexpr int GEMM_OUT_BOX = GEMM_BM * 64 * 2;   // one 64-column TMA store box of a tile, 16 KiB
-constexpr int GEMM_OUT_OFFSET = GEMM_STAGES * GEMM_STAGE_BYTES;   // [consumer][2 boxes] staging tiles
-constexpr int GEMM_BAR_OFFSET = GEMM_OUT_OFFSET + 2 * 2 * GEMM_OUT_BOX;
-constexpr int GEMM_SMEM_BYTES = GEMM_BAR_OFFSET + 16 * GEMM_STAGES + 1024;   // + slack to align to 1024 B
-static_assert(GEMM_SMEM_BYTES <= 232448, "shared memory of one SM");
 // named barriers: GEMM_BAR_TURN + w = consumer w may issue its main loop; GEMM_BAR_STAGE + w = consumer w's
 // staging tile is free / written; GEMM_BAR_NF4 = the NF4 producers have dequantised a k-block
 constexpr int GEMM_BAR_TURN = 1, GEMM_BAR_STAGE = 3, GEMM_BAR_NF4 = 5;
@@ -67,9 +70,10 @@ constexpr int GEMM_NF4_RAW = 4;                                    // raw ring s
 constexpr int GEMM_NF4_CODE_BYTES = GEMM_BN * GEMM_BK / 2;         // 128 rows x 32 bytes
 constexpr int GEMM_NF4_RAW_BYTES = GEMM_NF4_CODE_BYTES + GEMM_BN * 4;   // + 128 fp32 scales
 
-// Shared-memory plan and register split of one instantiation: [stages][output staging][raw ring][mbarriers]
-// [code table].  The 16-bit 128-wide plan is the constants above.  At BN = 192 a stage is 40 KiB and each
-// consumer's staging tile three 16 KiB store boxes, which leaves room for three stages.
+// Shared-memory plan and register split of one instantiation: [stages][output staging][bias slots][raw ring]
+// [mbarriers][code table].  At BN = 128 a stage is 32 KiB and each consumer's staging tile two 16 KiB store boxes;
+// at BN = 192 a stage is 40 KiB and a staging tile three boxes, which leaves room for three stages.  A bias slot
+// holds the BN fp32 bias values of the consumer's current tile.
 template <bool NF4, int BN = GEMM_BN>
 struct GemmPlan {
   static_assert(BN == 128 || BN == 192, "tile widths");
@@ -78,7 +82,8 @@ struct GemmPlan {
   static constexpr int OUT_BOXES = BN / 64;   // 64-column TMA store boxes per tile
   static constexpr int STAGES = NF4 ? 4 : BN == 192 ? 3 : GEMM_STAGES;
   static constexpr int OUT_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int RAW_OFFSET = OUT_OFFSET + 2 * OUT_BOXES * GEMM_OUT_BOX;
+  static constexpr int BIAS_OFFSET = OUT_OFFSET + 2 * OUT_BOXES * GEMM_OUT_BOX;   // [consumer][BN] fp32
+  static constexpr int RAW_OFFSET = BIAS_OFFSET + 2 * BN * 4;
   static constexpr int BAR_OFFSET = RAW_OFFSET + (NF4 ? GEMM_NF4_RAW * GEMM_NF4_RAW_BYTES : 0);
   // full[STAGES], empty[STAGES], then (NF4) raw_full[GEMM_NF4_RAW]
   static constexpr int TABLE_OFFSET = BAR_OFFSET + 16 * STAGES + (NF4 ? 8 * GEMM_NF4_RAW : 0);
@@ -92,8 +97,7 @@ struct GemmPlan {
   static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= GEMM_THREADS * 168, "registers the CTA holds");
   static_assert(SMEM_BYTES <= 232448, "shared memory of one SM");
 };
-static_assert(GemmPlan<false>::SMEM_BYTES == GEMM_SMEM_BYTES && GemmPlan<false>::BAR_OFFSET == GEMM_BAR_OFFSET &&
-              GemmPlan<false>::STAGE_BYTES == GEMM_STAGE_BYTES, "the 16-bit plan");
+static_assert(GemmPlan<false>::STAGE_BYTES == GEMM_STAGE_BYTES, "the 16-bit plan");
 
 // bitsandbytes' NF4 code values (embed/encoders/nf4.py: NF4_CODE) as fp32 bit patterns
 __constant__ uint32_t kNf4CodeBits[16] = {
@@ -143,7 +147,8 @@ __device__ __forceinline__ float silu(float x) {
 
 // profiling aid (b2e_debug_set_clock_buffer): CTA 0 of the TL instantiation records clock64() once per
 // K block in the producer ([0][n], after issuing the loads) and in the first consumer warpgroup ([1][n], when
-// the block's MMAs have been retired); 4 x 256 int64
+// the block's MMAs have been retired), and at the start and end of each epilogue of the first consumer ([2][e]
+// when its accumulators are final, [3][e] after its TMA store is issued; e = its e-th tile); 4 x 256 int64
 __device__ long long* g_gemm_clock = nullptr;
 
 // The tiles of CTA blockIdx.x: first, first + stride, ... (count of them) of the linear tile index, N tiles
@@ -180,6 +185,21 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
 }
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float2 v) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
+}
+// four 8 x 8 b16 matrices: lanes 8i .. 8i + 7 give the 16-byte row addresses of matrix i, and register i of lane l
+// holds row l / 4, columns 2 (l % 4) + {0, 1} of matrix i -- the layout of a wgmma accumulator's 8-column group
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
 }
 
 // The NF4 producer warpgroup (all 128 threads; thread p dequantises W row p of every tile).  Thread 0 also issues
@@ -324,6 +344,14 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   const int quad = t & 3;
   const int r_lo = 16 * (t >> 5) + ((t & 31) >> 2);   // row of acc[h][4j + {0,1}] in its 64-row half
   const uint32_t stg = sb + P::OUT_OFFSET + wg * (P::OUT_BOXES * GEMM_OUT_BOX);
+  const uint32_t bias_slot = sb + P::BIAS_OFFSET + wg * (BN * 4);
+  // stmatrix row address of this lane in the staging tile, for the four matrices (group j0 + i / 2, rows + 8 (i % 2))
+  // of groups j0, j0 + 1 (j0 even) at j0 = 0: lane 8i + k gives row 16 (t / 32) + 8 (i % 2) + k, whose unit
+  // (i / 2) sits at (i / 2) ^ k.  The staging tile is 1024-byte aligned, so the swizzle of a later j0 is an XOR of
+  // this address with ((j0 & 7) << 4).
+  const int lane = t & 31;
+  const uint32_t stm_addr = stg + (16 * (t >> 5) + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128 +
+                            ((((lane >> 4) ^ lane) & 7) << 4);
   int retired = 0;
   // Turn i (the CTA's i-th tile) belongs to consumer i % 2.  The hand-over into turn i (1 <= i < count) is one
   // arrive by the consumer of turn i - 1 after issuing its main loop and one sync by the consumer of turn i
@@ -331,6 +359,11 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   for (int i = wg; i < tl.count; i += 2) {
     const int tile = tl.first + i * tl.stride;
     const int m0 = (tile / tl.n_tiles) * GEMM_BM, n_blk = tile % tl.n_tiles;
+    // the tile's bias, loaded here and written to the consumer's slot after the main loop (threads t < BN / 2, one
+    // pair each); without a bias the slot holds -0, which leaves every sum as it is, -0 included
+    float2 bias_pair = make_float2(-0.0f, -0.0f);
+    if constexpr (!epi_is_glu(EPI))
+      if (bias != nullptr && t < BN / 2) bias_pair = __ldg(reinterpret_cast<const float2*>(bias + n_blk * BN) + t);
     float acc[2][BN / 2];   // rows [64 h, 64 h + 64) of the tile
 #pragma unroll
     for (int x = 0; x < BN / 2; ++x) acc[0][x] = acc[1][x] = 0.0f;
@@ -376,74 +409,90 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
     reg_fence(acc[0]);
     reg_fence(acc[1]);
     if (t == 0) mbar_arrive(empty_bar + 8u * prev);
+    if (TL && clk != nullptr && wg == 0 && t == 0 && i / 2 < 256) clk[512 + i / 2] = clock64();
+    // Every thread of this warpgroup left the slot's previous tile behind before the turn sync above (i >= 2).
+    if constexpr (!epi_is_glu(EPI))
+      if (t < BN / 2) st_shared_f32x2(bias_slot + 8 * t, bias_pair);
 
-    // Epilogue.  A tile inside the device rows goes out through the staging tile (128-byte swizzle, the
-    // layout of the store map: 16-byte unit u of row r sits at unit u ^ (r & 7), so that the eight rows of a
-    // warp's store hit distinct banks) and TMA; a tile crossing M stores its rows from registers.
+    // Epilogue: fp32 acc (+ bias, then erf-GELU | + residual | the gated activation), rounded to h16 pairs.  A tile
+    // inside the device rows goes out through the staging tile (128-byte swizzle, the layout of the store map:
+    // 16-byte unit u of row r sits at unit u ^ (r & 7), so that the eight rows of a matrix hit distinct banks) and
+    // TMA, with no test or global address inside its element loop; the last row tile crossing M stores its rows
+    // from registers.
     const bool staged = m0 + GEMM_BM <= M;
+    if (staged && t == 0) tma_store_wait_read<0>();   // the previous tile's stores have read the staging tile
+    named_bar_sync(GEMM_BAR_STAGE + wg, 128);          // ... and the bias slot is written
+    // the output pair of acc[h][4j + 2 half + {0, 1}]: row 64 h + r_lo + 8 half, columns 8 j + 2 quad + {0, 1} of
+    // the tile (the gated epilogues: of the 64-column output block); b = the bias pair of group j, res = the
+    // residual pair
+    auto out_pair = [&](int h, int j, int half, float2 b, uint32_t res) -> uint32_t {
+      if constexpr (epi_is_glu(EPI)) {
+        const float g0 = acc[h][4 * j + 2 * half], g1 = acc[h][4 * j + 2 * half + 1];
+        const float u0 = acc[h][4 * (j + 8) + 2 * half], u1 = acc[h][4 * (j + 8) + 2 * half + 1];
+        if constexpr (EPI == EPI_GEGLU) return pack_h16x2(gelu_erf_fast(g0) * u0, gelu_erf_fast(g1) * u1);
+        else return pack_h16x2(silu(g0) * u0, silu(g1) * u1);
+      } else {
+        float v0 = acc[h][4 * j + 2 * half] + b.x, v1 = acc[h][4 * j + 2 * half + 1] + b.y;
+        if constexpr (EPI == EPI_BIAS_GELU) {
+          v0 = gelu_erf_fast(v0);
+          v1 = gelu_erf_fast(v1);
+        }
+        if constexpr (EPI == EPI_BIAS_RESID) {
+          const float2 rv = unpack_h16x2(res);
+          v0 += rv.x;
+          v1 += rv.y;
+        }
+        return pack_h16x2(v0, v1);
+      }
+    };
+    constexpr int GROUPS = epi_is_glu(EPI) ? 8 : BN / 8;   // 8-column output groups
+    const int n_out = epi_is_glu(EPI) ? N / 2 : N;
+    const int col0 = n_blk * (epi_is_glu(EPI) ? GEMM_BN / 2 : BN) + 2 * quad;
+    const h16* res_row = EPI == EPI_BIAS_RESID ? resid + static_cast<size_t>(m0 + r_lo) * N + col0 : nullptr;
     if (staged) {
-      if (t == 0) tma_store_wait_read<0>();   // the previous tile's stores have read the staging tile
-      named_bar_sync(GEMM_BAR_STAGE + wg, 128);
-    }
-    if constexpr (epi_is_glu(EPI)) {
-      const int n_out = N / 2;
+      // Groups j0, j0 + 1 of both 64-row halves per step: 16 independent pairs, two stmatrix.x4, and the
+      // accumulators of the step die as it is written.  The next step's bias (and residual) pairs are read first.
+      const size_t rs8 = static_cast<size_t>(8) * N;   // residual rows 8 apart
+      float2 b[2][2];
+      uint32_t res[2][2][2][2] = {};   // [buffer][h][group of the step][half]
+      auto load_step = [&](int s, int buf) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
+        for (int g = 0; g < 2; ++g) {
+          b[buf][g] = epi_is_glu(EPI) ? make_float2(0.0f, 0.0f) : ld_shared_f32x2(bias_slot + 4 * (8 * (2 * s + g) + 2 * quad));
+          if constexpr (EPI == EPI_BIAS_RESID)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int half = 0; half < 2; ++half)
+                res[buf][h][g][half] =
+                    __ldg(reinterpret_cast<const uint32_t*>(res_row + rs8 * (8 * h + half) + 8 * (2 * s + g)));
+        }
+      };
+      load_step(0, 0);
+#pragma unroll
+      for (int s = 0; s < GROUPS / 2; ++s) {
+        if (s + 1 < GROUPS / 2) load_step(s + 1, (s + 1) & 1);
+        const int j0 = 2 * s, buf = s & 1;
+        const uint32_t addr = (stm_addr ^ ((j0 & 7) << 4)) + (j0 >> 3) * GEMM_OUT_BOX;
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const int r = 64 * h + r_lo + 8 * half;
-            const float g0 = acc[h][4 * j + 2 * half], g1 = acc[h][4 * j + 2 * half + 1];
-            const float u0 = acc[h][4 * (j + 8) + 2 * half], u1 = acc[h][4 * (j + 8) + 2 * half + 1];
-            float v0, v1;
-            if (EPI == EPI_GEGLU) {
-              v0 = gelu_erf_fast(g0) * u0;
-              v1 = gelu_erf_fast(g1) * u1;
-            } else {
-              v0 = silu(g0) * u0;
-              v1 = silu(g1) * u1;
-            }
-            if (staged)
-              st_shared_u32(stg + r * 128 + ((j ^ (r & 7)) << 4) + 4 * quad, pack_h16x2(v0, v1));
-            else if (m0 + r < M)
-              *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(m0 + r) * n_out + n_blk * (GEMM_BN / 2) +
-                                           8 * j + 2 * quad) = pack_h16x2(v0, v1);
-          }
+          stmatrix_x4(addr + h * 64 * 128, out_pair(h, j0, 0, b[buf][0], res[buf][h][0][0]),
+                      out_pair(h, j0, 1, b[buf][0], res[buf][h][0][1]), out_pair(h, j0 + 1, 0, b[buf][1], res[buf][h][1][0]),
+                      out_pair(h, j0 + 1, 1, b[buf][1], res[buf][h][1][1]));
+      }
     } else {
-      const int col0 = n_blk * BN + 2 * quad;
-      // ascending j: the eight accumulators of group j die as it is written, which makes room for the bias pairs
-      // of the groups ahead
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const float2 b = bias != nullptr ? __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * j))
-                                         : make_float2(0.0f, 0.0f);
+      for (int j = 0; j < GROUPS; ++j) {
+        const float2 b = epi_is_glu(EPI) ? make_float2(0.0f, 0.0f) : ld_shared_f32x2(bias_slot + 4 * (8 * j + 2 * quad));
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int half = 0; half < 2; ++half) {
             const int r = 64 * h + r_lo + 8 * half;
-            if (!staged && m0 + r >= M) continue;
-            float v0 = acc[h][4 * j + 2 * half], v1 = acc[h][4 * j + 2 * half + 1];
-            if (bias != nullptr) {
-              v0 += b.x;
-              v1 += b.y;
-            }
-            if (EPI == EPI_BIAS_GELU) {
-              v0 = gelu_erf_fast(v0);
-              v1 = gelu_erf_fast(v1);
-            }
-            const size_t off = static_cast<size_t>(m0 + r) * N + col0 + 8 * j;
-            if (EPI == EPI_BIAS_RESID) {
-              const float2 rv = unpack_h16x2(*reinterpret_cast<const uint32_t*>(resid + off));
-              v0 += rv.x;
-              v1 += rv.y;
-            }
-            if (staged)
-              st_shared_u32(stg + (j >> 3) * GEMM_OUT_BOX + r * 128 + (((j & 7) ^ (r & 7)) << 4) + 4 * quad,
-                            pack_h16x2(v0, v1));
-            else
-              *reinterpret_cast<uint32_t*>(out + off) = pack_h16x2(v0, v1);
+            if (m0 + r >= M) continue;
+            const size_t off = static_cast<size_t>(m0 + r) * n_out + col0 + 8 * j;
+            const uint32_t res = EPI == EPI_BIAS_RESID ? *reinterpret_cast<const uint32_t*>(resid + off) : 0u;
+            *reinterpret_cast<uint32_t*>(out + off) = out_pair(h, j, half, b, res);
           }
       }
     }
@@ -460,6 +509,7 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
         tma_store_commit();
       }
     }
+    if (TL && clk != nullptr && wg == 0 && t == 0 && i / 2 < 256) clk[768 + i / 2] = clock64();
   }
   if (t == 0) tma_store_wait_all();   // the stores have read shared memory before the CTA leaves
 }

@@ -24,8 +24,9 @@ int b2e_debug_set_att3_clock(void* device_buffer);
 /* which instantiated variant of the head_dim-64 attention kernel the next launches use (also B2E_ATT3; -1 = the
  * environment / built-in default) */
 int b2e_debug_set_att3_variant(int variant);
-/* device buffer of 4 x 256 int64 filled with clock64() stamps by CTA (0, 0) of the bias GEMM while set (the
- * timeline instantiation runs instead of the production one); NULL switches it off */
+/* device buffer of 4 x 256 int64 filled with clock64() stamps by CTA (0, 0) of the bias and bias + GELU GEMMs while
+ * set (the timeline instantiation runs instead of the production one; csrc/gemm.cuh: g_gemm_clock); NULL switches
+ * it off */
 int b2e_debug_set_clock_buffer(void* device_buffer);
 /* tile width of the GEMM (csrc/gemm.cuh) for the W maps built from now on -- encoder handles created and
  * b2e_gemm_h16 calls made after it: 128 or 192 forces it wherever the 192-wide kernel exists (16-bit weights, no
