@@ -95,6 +95,7 @@ DEBUG_EXPORTS = (
     'b2e_debug_gemm_rows',
     'b2e_debug_topk_tc_fell_back',
     'b2e_debug_attention_packed',
+    'b2e_debug_rotary',
 )
 
 
@@ -383,6 +384,23 @@ def attention_packed(qkv: torch.Tensor, attention_mask: torch.Tensor, batch: int
                                              heads, kv_heads, head_dim, window, int(causal),
                                              stream_ptr(qkv.device)), lib)
     return ctx
+
+
+def debug_rotary_(enc, layer: int, qkv: torch.Tensor, attention_mask: torch.Tensor) -> torch.Tensor:
+    """Debug hook: the rotary step of ``layer`` of encoder ``enc`` (embed.encoders.native), in place on qkv
+    [B*S, q | k | v columns] in the token layout the encoder derives from ``attention_mask`` (see attention_packed)."""
+    lib = enc._lib
+    _cuda_contig(qkv, 'qkv'), _cuda_contig(attention_mask, 'attention_mask')
+    if attention_mask.dtype != torch.int64:
+        raise NativeError('attention_mask must be int64')
+    b, s = attention_mask.shape
+    if qkv.shape[0] != b * s or qkv.dtype != STORAGE_TORCH_DTYPE[enc.storage]:
+        raise NativeError(f'debug_rotary_: qkv must be [B*S = {b * s}, cols] in the encoder storage type')
+    lib.b2e_debug_rotary.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    with torch.cuda.device(qkv.device):
+        check(lib.b2e_debug_rotary(enc._handle, layer, qkv.data_ptr(), attention_mask.data_ptr(), b, s,
+                                   stream_ptr(qkv.device)), lib)
+    return qkv
 
 
 def qk_norm_rope_(qkv: torch.Tensor, q_gamma: torch.Tensor, k_gamma: torch.Tensor, cos: torch.Tensor,

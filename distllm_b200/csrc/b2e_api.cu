@@ -753,6 +753,36 @@ int trunk_prologue(B2EEncoder* e, const int64_t* mask, int B, int S, cudaStream_
   return make_tmap_h16(&tm->qkv, e->qkv, M, e->qkv_cols(), AT_KC, d.head_dim);
 }
 
+// The rotary step of layer l, in place on qkv [M, qkv_cols()] in the token layout `lay` (rows from lay.t_real on are
+// not touched): ESM-2 rope_halves<16> (head_dim 32) or <32> over its q and k heads, ModernBERT rope_halves<32> with the
+// full-attention (l % global_every == 0) or the sliding-attention table, Mistral rope_halves<64>, Qwen3 the per-head
+// q / k RMSNorm fused with the rotation.  The trunks and b2e_debug_rotary launch it.
+void launch_rotary(B2EEncoder* e, int l, h16* qkv, int M, int S, cudaStream_t st, const SeqLayout& lay) {
+  const B2EModelDesc& d = e->desc;
+  if (is_decoder(d.arch)) {
+    const int n_rot = d.heads + d.kv_heads;   // q heads and k heads are adjacent columns of qkv
+    const unsigned grid = (unsigned)(((long long)M * n_rot * 8 + 255) / 256);
+    if (d.arch == B2E_ARCH_QWEN3)
+      qk_rmsnorm_rope_kernel<<<grid, 256, 0, st>>>(qkv, (const float*)e->slot(l, 6), (const float*)e->slot(l, 7),
+                                                   e->rope_cos, e->rope_sin, M, S, d.heads, d.kv_heads, e->qkv_cols(),
+                                                   d.eps, lay.t_real, lay.tok_src);
+    else
+      rope_halves_kernel<64><<<grid, 256, 0, st>>>(qkv, e->rope_cos, e->rope_sin, M, S, n_rot, e->qkv_cols(),
+                                                   lay.t_real, lay.tok_src);
+    return;
+  }
+  const long long rope_work = (long long)M * d.heads * 2;
+  const bool global = d.arch != B2E_ARCH_MODERNBERT || (l % d.global_every) == 0;
+  const float* cos_t = global ? e->rope_cos : e->rope_cos2;
+  const float* sin_t = global ? e->rope_sin : e->rope_sin2;
+  if (d.head_dim == 32)   // two threads per head of 2 x 16 frequencies
+    rope_halves_kernel<16><<<(unsigned)((rope_work * 2 + 255) / 256), 256, 0, st>>>(
+        qkv, cos_t, sin_t, M, S, 2 * d.heads, 3 * d.hidden, lay.t_real, lay.tok_src);
+  else
+    rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
+        qkv, cos_t, sin_t, M, S, 2 * d.heads, 3 * d.hidden, lay.t_real, lay.tok_src);
+}
+
 // Layers 0..L-1 up to (and including) the last FFN-down GEMM: leaves the pre-LayerNorm residual sum
 // of the final layer split as e->tmp (FFN-down output + bias) and e->hidden (the residual it still has
 // to be added to); every earlier LayerNorm output lives in e->hidden.
@@ -822,18 +852,11 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const 
   DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      e->xres, nullptr, (const float*)e->slot(0, 0), (const float*)e->slot(0, 1), e->hidden,
                      M, d.eps, lay.t_real)));
-  const long long rope_work = (long long)M * d.heads * 2;
   for (int l = 0; l < L; ++l) {
     if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, (const float*)e->slot(l, 3), nullptr, M,
                           3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    if (d.head_dim == 32) {   // two threads per head of 2 x 16 frequencies
-      rope_halves_kernel<16><<<(unsigned)((rope_work * 2 + 255) / 256), 256, 0, st>>>(
-          e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
-    } else {
-      rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
-          e->qkv, e->rope_cos, e->rope_sin, M, S, 2 * d.heads, 3 * H, lay.t_real, lay.tok_src);
-    }
+    launch_rotary(e, l, e->qkv, M, S, st, lay);
     if ((rc = launch_attention_bidir(tm.qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
       return rc;
     if ((rc = launch_gemm(tm.ctx, e->tm_wo[l], e->tmp, (const float*)e->slot(l, 5), nullptr, M, H, H,
@@ -878,19 +901,10 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
 
   DISPATCH_H(H, (add_rmsnorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                      e->xres, nullptr, (const float*)e->slot(0, 0), e->hidden, M, d.eps, lay.t_real)));
-  const int n_rot = d.heads + d.kv_heads;   // q heads and k heads are adjacent columns of qkv
-  const long long rope_work = (long long)M * n_rot;
   for (int l = 0; l < L; ++l) {
     if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, QC, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    if (d.arch == B2E_ARCH_QWEN3) {
-      qk_rmsnorm_rope_kernel<<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
-          e->qkv, (const float*)e->slot(l, 6), (const float*)e->slot(l, 7), e->rope_cos, e->rope_sin, M, S, d.heads,
-          d.kv_heads, QC, d.eps, lay.t_real, lay.tok_src);
-    } else {
-      rope_halves_kernel<64><<<(unsigned)((rope_work * 8 + 255) / 256), 256, 0, st>>>(
-          e->qkv, e->rope_cos, e->rope_sin, M, S, n_rot, QC, lay.t_real, lay.tok_src);
-    }
+    launch_rotary(e, l, e->qkv, M, S, st, lay);
     if ((rc = launch_attention_causal_d128(e->qkv, e->attn, e->ctx, B, S, d.heads, d.kv_heads,
                                            d.sliding_window, st, lay)))
       return rc;
@@ -929,7 +943,6 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
   CUDA_TRY(cudaGetLastError());
   TrunkMaps tm;
   if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
-  const long long rope_work = (long long)M * d.heads * 2;
   for (int l = 0; l < L; ++l) {
     const bool global = (l % d.global_every) == 0;
     if (l > 0) {
@@ -939,9 +952,7 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
     }
     if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, 3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
-    rope_halves_kernel<32><<<(unsigned)((rope_work * 4 + 255) / 256), 256, 0, st>>>(
-        e->qkv, global ? e->rope_cos : e->rope_cos2, global ? e->rope_sin : e->rope_sin2, M, S, 2 * d.heads,
-        3 * H, lay.t_real, lay.tok_src);
+    launch_rotary(e, l, e->qkv, M, S, st, lay);
     if ((rc = launch_attention(tm.qkv, e->attn, e->ctx, B, S, d.heads, st,
                                global ? 0 : d.sliding_window, lay)))
       return rc;
@@ -1632,6 +1643,24 @@ int b2e_attention_causal_d128(const void* qkv, const int64_t* mask, void* ctx, i
 // The encoder's attention step in its own token layout: pack_prepare decides the layout from the mask (attended
 // tokens back to back when every row is a non-empty prefix, else the identity layout), then the same launch as the
 // trunks, on tensor maps spanning B*S rows.  qkv / ctx rows are in that layout.
+// The handle's rotary step of `layer` (launch_rotary), in place on the caller's qkv [B*S, qkv columns of the
+// family], in the token layout the encoder derives from the mask (pack_prepare, b2e_debug_set_packing).
+int b2e_debug_rotary(B2EEncoder* e, int layer, void* qkv, const int64_t* mask, int B, int S, void* stream) {
+  int rc;
+  if ((rc = validate_batch(e, B, S))) return rc;
+  if (!qkv || !mask) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (e->desc.arch == B2E_ARCH_BERT) return fail(B2E_ERR_INVALID, "debug_rotary: BERT has no rotary step");
+  if (layer < 0 || layer >= e->desc.num_layers)
+    return fail(B2E_ERR_INVALID, "debug_rotary: layer %d of %d", layer, e->desc.num_layers);
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = e->pack.ensure(B, (size_t)B * S))) return rc;
+  SeqLayout lay;
+  if ((rc = pack_prepare(e->pack, mask, B, S, packing_enabled(), st, &lay))) return rc;
+  launch_rotary(e, layer, (h16*)qkv, B * S, S, st, lay);
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
+}
+
 int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
                                int kv_heads, int head_dim, int window, int causal, void* stream) {
   if (!qkv || !mask || !ctx) return fail(B2E_ERR_INVALID, "null tensor pointer");

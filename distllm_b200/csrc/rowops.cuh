@@ -87,7 +87,9 @@ __device__ __forceinline__ void warp_layernorm(float (&x)[row_passes(H)][8], con
   for (int v = 0; v < NV; ++v)
 #pragma unroll
     for (int e = 0; e < 8; ++e) s += x[v][e];
-  const float mean = warp_sum(s) * inv_h;
+  // rounded on its own: contracted into x - mean (one fma), a constant row c at H = 3 * 2^k or 5 * 2^k, where
+  // H * fl(1/H) != 1, leaves d = -c * 2^-25 or -c * 2^-26 instead of 0, which eps = 1e-12 scales up to ~0.03 c
+  const float mean = __fmul_rn(warp_sum(s), inv_h);
   float ss = 0.0f;
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
@@ -403,17 +405,18 @@ __global__ void pool_finalize_kernel(const float* __restrict__ part, const float
     row[c] = v;
     ss = fmaf(v, v, ss);
   }
-  float scale = 1.0f;
+  float norm = 1.0f;
   if (l2_normalize) {
     ss = warp_sum(ss);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
     __syncthreads();
     float tot = 0.0f;
     for (int i = 0; i < static_cast<int>(blockDim.x >> 5); ++i) tot += red[i];
-    scale = 1.0f / fmaxf(sqrtf(tot), 1e-12f);
+    norm = fmaxf(sqrtf(tot), 1e-12f);
   }
+  // a division, as F.normalize does: x * (1 / norm) differs from x / norm by one ulp in about a third of elements
   for (int c = threadIdx.x; c < H; c += blockDim.x)
-    out[static_cast<size_t>(b) * H + c] = row[c] * scale;
+    out[static_cast<size_t>(b) * H + c] = l2_normalize ? row[c] / norm : row[c];
 }
 
 // out[b,:] = in[b, idx[b], :] as fp32 (last_token.py:33-39), optional L2 normalise done separately.
@@ -440,10 +443,10 @@ __global__ void l2_normalize_kernel(float* __restrict__ x, int N, int H) {
     const float4 v = *reinterpret_cast<const float4*>(p + c);
     ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
   }
-  const float scale = 1.0f / fmaxf(sqrtf(warp_sum(ss)), 1e-12f);
+  const float norm = fmaxf(sqrtf(warp_sum(ss)), 1e-12f);   // divided by, as F.normalize does (pool_finalize_kernel)
   for (int c = lane * 4; c < H; c += 128) {
     float4 v = *reinterpret_cast<float4*>(p + c);
-    v.x *= scale; v.y *= scale; v.z *= scale; v.w *= scale;
+    v.x /= norm; v.y /= norm; v.z /= norm; v.w /= norm;
     *reinterpret_cast<float4*>(p + c) = v;
   }
 }

@@ -158,6 +158,8 @@ int b2e_pool_mean(const void* hidden, int dtype, int64_t* attention_mask, int B,
                   int pool_kind, int quirk_mutate, float* out, void* stream);
 int b2e_pool_last_token(const void* hidden, int dtype, const int64_t* attention_mask, int B, int S,
                         int H, float* out, void* stream);
+/* In place, per row: x / max(||x||_2, 1e-12), divided as F.normalize divides (so is l2_normalize of
+ * b2e_encode_pooled / b2e_embed_host). */
 int b2e_l2_normalize(float* x, int64_t n_rows, int H, void* stream);
 
 /* out[i] = 1 - cos(emb[i], emb[i+1]) for i in [0, n_rows-1); pairs with doc_id[i] != doc_id[i+1]

@@ -52,6 +52,12 @@ int b2e_debug_topk_tc_fell_back(int* out);
  * head_dim 128 (window > 0: q - k < window).  The head_dim-64 kernel is b2e_debug_set_att3_variant's. */
 int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
                                int kv_heads, int head_dim, int window, int causal, void* stream);
+/* the encoder's rotary step of `layer`, in place on qkv (B*S rows of the family's q | k | v columns, 16-bit storage)
+ * in the token layout it derives from the mask, as b2e_debug_attention_packed: ESM-2 and ModernBERT (its full or
+ * sliding table by layer) rotate the q and k heads, Mistral the q and k heads, Qwen3 normalises each q / k head with
+ * the layer's q_norm / k_norm before rotating it.  Rows past the last attended token (packed layout) and the v
+ * heads are not touched. */
+int b2e_debug_rotary(struct B2EEncoder* enc, int layer, void* qkv, const int64_t* mask, int B, int S, void* stream);
 
 #ifdef __cplusplus
 }
