@@ -60,6 +60,7 @@ EXPORTS = (
     'b2e_check_model',
     'b2e_encoder_create',
     'b2e_encoder_create_nf4',
+    'b2e_encoder_create_nf4_lora',
     'b2e_encoder_destroy',
     'b2e_workspace_bytes',
     'b2e_encode',
@@ -71,6 +72,7 @@ EXPORTS = (
     'b2e_adjacent_cosine_dist',
     'b2e_gemm_h16',
     'b2e_gemm_nf4',
+    'b2e_gemm_nf4_lora',
     'b2e_attention_d64',
     'b2e_attention_d32',
     'b2e_attention_d64_window',
@@ -93,6 +95,7 @@ DEBUG_EXPORTS = (
     'b2e_debug_set_gemm_bn',
     'b2e_debug_gemm_bn',
     'b2e_debug_gemm_rows',
+    'b2e_debug_gemm_nf4_lora_rows',
     'b2e_debug_topk_tc_fell_back',
     'b2e_debug_attention_packed',
     'b2e_debug_rotary',
@@ -146,6 +149,9 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_encoder_create_nf4.restype = i32
     lib.b2e_encoder_create_nf4.argtypes = [C.POINTER(ModelDesc), C.POINTER(vp), i32, C.POINTER(vp), i32, i32,
                                            C.POINTER(vp)]
+    lib.b2e_encoder_create_nf4_lora.restype = i32
+    lib.b2e_encoder_create_nf4_lora.argtypes = [C.POINTER(ModelDesc), C.POINTER(vp), i32, C.POINTER(vp), i32,
+                                                C.POINTER(vp), C.POINTER(vp), C.POINTER(i32), i32, i32, C.POINTER(vp)]
     lib.b2e_encoder_destroy.restype = None
     lib.b2e_encoder_destroy.argtypes = [vp]
     lib.b2e_workspace_bytes.restype = i64
@@ -168,6 +174,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_gemm_h16.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b2e_gemm_nf4.restype = i32
     lib.b2e_gemm_nf4.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.b2e_gemm_nf4_lora.restype = i32
+    lib.b2e_gemm_nf4_lora.argtypes = [vp, vp, vp, vp, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.b2e_attention_d64.restype = i32
     lib.b2e_attention_d64.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
     lib.b2e_attention_d32.restype = i32
@@ -304,6 +312,37 @@ def gemm_nf4(
     with torch.cuda.device(a.device):
         check(lib.b2e_gemm_nf4(a.data_ptr(), codes.data_ptr(), absmax.data_ptr(), _ptr(bias), _ptr(resid),
                                out.data_ptr(), m, n, k, epilogue, stream_ptr(a.device)), lib)
+    return out
+
+
+def gemm_nf4_lora(
+    a: torch.Tensor,
+    codes: torch.Tensor,
+    absmax: torch.Tensor,
+    u: torch.Tensor,
+    b_cat: torch.Tensor,
+    bias: torch.Tensor | None,
+    resid: torch.Tensor | None = None,
+    epilogue: int = EPI_BIAS,
+) -> torch.Tensor:
+    """:func:`gemm_nf4` plus the low-rank term ``u[:, :R] @ b_cat.T`` inside the same sum (R = ``b_cat.shape[1]``, a
+    multiple of 64; ``u`` [M, >= R] may be wider, its row stride is its width).  Equals bit for bit :func:`gemm_h16`
+    on ``[a | u[:, :R]]`` and ``[dequant(W) | b_cat]``."""
+    lib = load(storage_of(a.dtype))
+    for t, what in ((a, 'a'), (codes, 'codes'), (absmax, 'absmax'), (u, 'u'), (b_cat, 'b_cat')):
+        _cuda_contig(t, what)
+    if bias is not None:
+        _cuda_contig(bias, 'bias')
+    m, k = a.shape
+    n, r = b_cat.shape
+    if u.dtype != a.dtype or b_cat.dtype != a.dtype or u.shape[0] != m:
+        raise NativeError(f'gemm_nf4_lora: u must be [{m}, >= R] and b_cat [N, R] in {a.dtype}')
+    n_out = n // 2 if epilogue in (EPI_SWIGLU, EPI_GEGLU) else n
+    out = torch.empty((m, n_out), dtype=a.dtype, device=a.device)
+    with torch.cuda.device(a.device):
+        check(lib.b2e_gemm_nf4_lora(a.data_ptr(), codes.data_ptr(), absmax.data_ptr(), u.data_ptr(), u.shape[1],
+                                    b_cat.data_ptr(), r, _ptr(bias), _ptr(resid), out.data_ptr(), m, n, k,
+                                    epilogue, stream_ptr(a.device)), lib)
     return out
 
 

@@ -7,6 +7,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -77,13 +78,13 @@ EncodeTiledFn get_encode_fn() {
 }
 
 // 2-D half row-major [rows, cols] tensor, box = 64 columns (128 B, swizzle-128B) x box_rows, or with box_cols = 32
-// 32 columns (64 B, swizzle-64B: the head_dim-32 attention boxes).
+// 32 columns (64 B, swizzle-64B: the head_dim-32 attention boxes).  ld: the row stride in elements (0: cols).
 int make_tmap_h16(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols,
-                   uint32_t box_rows, uint32_t box_cols = 64) {
+                   uint32_t box_rows, uint32_t box_cols = 64, uint64_t ld = 0) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return fail(B2E_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 2};
+  cuuint64_t strides[1] = {(ld ? ld : cols) * 2};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(tm, B2E_TMAP_DTYPE, 2, const_cast<void*>(base), dims, strides,
@@ -221,10 +222,24 @@ int gemm_bn(int N, int epi, bool nf4) {
 // The W operand of a GEMM: a 16-bit [N,K] map (box 64 x bn), or with absmax set the NF4 code map
 // (make_tmap_codes) and the block scales [K/64, N] it is dequantised with.  `bn` is the tile width the map was
 // built for; the launch runs the kernel of that width.
+struct GemmLora;
 struct GemmW {
   CUtensorMap tm;
   const float* absmax = nullptr;
   int bn = GEMM_BN;
+  const GemmLora* lora = nullptr;   // NF4 only: the slot's low-rank term, run as extra k-blocks (gemm_nf4_lora_kernel)
+};
+
+// The low-rank term U . B_cat^T of an NF4 slot, U = X . A_cat^T (embed/encoders/weights.py: lora_slot_factors).
+// With u_ws set, launch_gemm first runs U's 16-bit GEMM from the slot's A operand into the handle's U workspace
+// [rows, r128] (*u_ws: the workspace moves when it grows); without, U is given (b2e_gemm_nf4_lora).
+struct GemmLora {
+  GemmW a;                       // A_cat [r128, K]: the W operand of U's GEMM
+  CUtensorMap tm_b;              // B_cat [N, 64 r_blocks], box 64 x 128
+  int r_blocks = 0, r128 = 0;    // R / 64; R rounded up to 128 (the rows of A_cat, the columns of U)
+  h16* const* u_ws = nullptr;
+  const void* u = nullptr;
+  int ldu = 0;
 };
 
 // epi: the B2E_EPI_* epilogue the GEMM will run with (it decides the tile width with N and the storage)
@@ -234,12 +249,39 @@ int make_gemm_w(GemmW* w, const void* base, const float* absmax, uint64_t rows, 
   return absmax ? make_tmap_codes(&w->tm, base, rows, cols / 2) : make_tmap_h16(&w->tm, base, rows, cols, w->bn);
 }
 
+// The LoRA factors of an [N, K] NF4 slot: A_cat 16-bit [round_up(R, 128), K], B_cat 16-bit [N, R], R % 64 == 0
+int make_gemm_lora(GemmLora* lo, const void* a_cat, const void* b_cat, int R, int N, int K) {
+  if (R <= 0 || R % GEMM_BK != 0) return fail(B2E_ERR_INVALID, "LoRA rank %d must be a positive multiple of 64", R);
+  lo->r_blocks = R / GEMM_BK;
+  lo->r128 = (R + 127) / 128 * 128;
+  int rc;
+  if ((rc = make_gemm_w(&lo->a, a_cat, nullptr, lo->r128, K, B2E_EPI_BIAS))) return rc;
+  return make_tmap_h16(&lo->tm_b, b_cat, N, R, GEMM_BN);
+}
+
 template <int EPI>
 int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const float* bias,
-                    const h16* resid, int M, int N, int K, cudaStream_t st, const int* m_dev) {
+                    const h16* resid, int M, int N, int K, cudaStream_t st, const int* m_dev,
+                    const CUtensorMap* tm_u = nullptr) {
   auto kern = gemm_h16_wgmma_kernel<EPI>;
   int smem = GemmPlan<false>::SMEM_BYTES;
   if (N % wb.bn != 0) return fail(B2E_ERR_INVALID, "gemm: N=%d is not a multiple of its W map's tile width %d", N, wb.bn);
+  if (wb.lora) {
+    int rc = ensure_smem_attr(gemm_nf4_lora_kernel<EPI>, GemmPlan<true>::SMEM_BYTES);
+    if (rc) return rc;
+    DeviceInfo dev;
+    if ((rc = current_device_info(&dev))) return rc;
+    const long long tiles = (long long)(N / GEMM_BN) * ((M + GEMM_BM - 1) / GEMM_BM);
+    if (tiles > 0x7fffffffLL) return fail(B2E_ERR_INVALID, "gemm: %lld output tiles exceed one grid", tiles);
+    CUtensorMap tm_out;
+    if ((rc = make_tmap_h16(&tm_out, out, M, epi_is_glu(EPI) ? N / 2 : N, GEMM_BM))) return rc;
+    const unsigned grid = (unsigned)(tiles < dev.sms ? tiles : dev.sms);
+    gemm_nf4_lora_kernel<EPI><<<grid, GEMM_THREADS, GemmPlan<true>::SMEM_BYTES, st>>>(
+        ta, wb.tm, tm_out, static_cast<h16*>(out), bias, resid, M, N, K, m_dev, wb.absmax, *tm_u, wb.lora->tm_b,
+        wb.lora->r_blocks);
+    CUDA_TRY(cudaGetLastError());
+    return B2E_OK;
+  }
   if (wb.absmax) {
     kern = gemm_h16_wgmma_kernel<EPI, false, true>;
     smem = GemmPlan<true>::SMEM_BYTES;
@@ -273,15 +315,30 @@ int launch_gemm_epi(const CUtensorMap& ta, const GemmW& wb, void* out, const flo
 
 // A map: [M,K] box 128 rows; W: see GemmW.
 // m_dev (nullable): device-resident row count <= M (packed token layout); M sizes the grid and the tensor maps.
+// A slot with a low-rank term (tb.lora) launches U's GEMM (when U lives in the handle's workspace) and then the
+// NF4 kernel with the tail k-blocks over U.
 int launch_gemm(const CUtensorMap& ta, const GemmW& tb, void* out, const float* bias,
                 const void* resid, int M, int N, int K, int epi, cudaStream_t st, const int* m_dev = nullptr) {
   const h16* r = static_cast<const h16*>(resid);
+  CUtensorMap tm_u;
+  if (tb.lora) {
+    const GemmLora& lo = *tb.lora;
+    const void* u = lo.u;
+    int ldu = lo.ldu, rc;
+    if (lo.u_ws) {
+      u = *lo.u_ws;
+      ldu = lo.r128;
+      if ((rc = launch_gemm_epi<EPI_BIAS>(ta, lo.a, const_cast<void*>(u), nullptr, nullptr, M, lo.r128, K, st, m_dev)))
+        return rc;
+    }
+    if ((rc = make_tmap_h16(&tm_u, u, M, (uint64_t)lo.r_blocks * GEMM_BK, GEMM_BM, 64, ldu))) return rc;
+  }
   switch (epi) {
-    case B2E_EPI_BIAS: return launch_gemm_epi<EPI_BIAS>(ta, tb, out, bias, r, M, N, K, st, m_dev);
-    case B2E_EPI_BIAS_GELU: return launch_gemm_epi<EPI_BIAS_GELU>(ta, tb, out, bias, r, M, N, K, st, m_dev);
-    case B2E_EPI_BIAS_RESID: return launch_gemm_epi<EPI_BIAS_RESID>(ta, tb, out, bias, r, M, N, K, st, m_dev);
-    case B2E_EPI_SWIGLU: return launch_gemm_epi<EPI_SWIGLU>(ta, tb, out, bias, r, M, N, K, st, m_dev);
-    case B2E_EPI_GEGLU: return launch_gemm_epi<EPI_GEGLU>(ta, tb, out, bias, r, M, N, K, st, m_dev);
+    case B2E_EPI_BIAS: return launch_gemm_epi<EPI_BIAS>(ta, tb, out, bias, r, M, N, K, st, m_dev, &tm_u);
+    case B2E_EPI_BIAS_GELU: return launch_gemm_epi<EPI_BIAS_GELU>(ta, tb, out, bias, r, M, N, K, st, m_dev, &tm_u);
+    case B2E_EPI_BIAS_RESID: return launch_gemm_epi<EPI_BIAS_RESID>(ta, tb, out, bias, r, M, N, K, st, m_dev, &tm_u);
+    case B2E_EPI_SWIGLU: return launch_gemm_epi<EPI_SWIGLU>(ta, tb, out, bias, r, M, N, K, st, m_dev, &tm_u);
+    case B2E_EPI_GEGLU: return launch_gemm_epi<EPI_GEGLU>(ta, tb, out, bias, r, M, N, K, st, m_dev, &tm_u);
   }
   return fail(B2E_ERR_INVALID, "unknown epilogue %d", epi);
 }
@@ -633,6 +690,11 @@ struct B2EEncoder {
   PackBuffers pack;
   // weight operands, one per layer: 16-bit maps, or (b2e_encoder_create_nf4) code maps with their block scales
   std::vector<GemmW> tm_wqkv, tm_wo, tm_w1, tm_w2;
+  // (b2e_encoder_create_nf4_lora) the low-rank terms, 4 per layer in the absmax order (r_blocks 0: none; sized
+  // once, the GemmW point into it), and U's workspace [tokens, lora_r128]
+  std::vector<GemmLora> lora;
+  int lora_r128 = 0;
+  DevBuf<h16> lora_u;
   // host-loop staging
   DevBuf<int64_t> stage_in;
   DevBuf<float> stage_out;
@@ -694,6 +756,7 @@ int ensure_workspace(B2EEncoder* e, int B, int S) {
     return rc;
   if (e->has_xres() && (rc = e->xres.grow(tokens * H, gen, true))) return rc;
   if (e->desc.arch == B2E_ARCH_ESM2 && (rc = e->tok_scale.grow(B, gen))) return rc;
+  if (e->lora_r128 && (rc = e->lora_u.grow(tokens * e->lora_r128, gen, true))) return rc;
   if ((rc = e->pack.ensure(B, tokens))) return rc;
   return e->pool.ensure(B, S, (size_t)B * pool_nsplit(S) * e->desc.hidden);
 }
@@ -1161,9 +1224,11 @@ int b2e_check_model(const B2EModelDesc* desc) {
 }
 
 namespace {
-// absmax: nullptr (16-bit matrices) or 4 * num_layers NF4 scale pointers (b2e_encoder_create_nf4)
+// absmax: nullptr (16-bit matrices) or 4 * num_layers NF4 scale pointers (b2e_encoder_create_nf4); lora_*: nullptr
+// or 4 * num_layers LoRA factors in the same order (b2e_encoder_create_nf4_lora)
 int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_weights, const float* const* absmax,
-                   int device, B2EEncoder** out) {
+                   int device, B2EEncoder** out, const void* const* lora_a = nullptr,
+                   const void* const* lora_b = nullptr, const int* lora_rank = nullptr) {
   if (!desc || !weights || !out) return fail(B2E_ERR_INVALID, "null argument");
   *out = nullptr;
   int rc;
@@ -1188,6 +1253,7 @@ int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_w
   const int L = desc->num_layers, H = desc->hidden, I = desc->intermediate;
   const int QC = e->qkv_cols(), CC = e->ctx_cols();
   e->tm_wqkv.resize(L); e->tm_wo.resize(L); e->tm_w1.resize(L); e->tm_w2.resize(L);
+  if (lora_rank) e->lora.resize(4 * (size_t)L);
   for (int l = 0; l < L; ++l) {
     const float* const* s = absmax ? absmax + 4 * l : nullptr;
     if ((rc = make_gemm_w(&e->tm_wqkv[l], e->slot(l, f.wqkv), s ? s[0] : nullptr, QC, H, B2E_EPI_BIAS)) ||
@@ -1196,6 +1262,21 @@ int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_w
         (rc = make_gemm_w(&e->tm_w2[l], e->slot(l, f.w2), s ? s[3] : nullptr, H, I, B2E_EPI_BIAS))) {
       b2e_encoder_destroy(e);
       return rc;
+    }
+    if (!lora_rank) continue;
+    GemmW* slots[4] = {&e->tm_wqkv[l], &e->tm_wo[l], &e->tm_w1[l], &e->tm_w2[l]};
+    const int rows[4] = {QC, H, f.w1_gated ? 2 * I : I, H}, cols[4] = {H, CC, H, I};
+    for (int j = 0; j < 4; ++j) {
+      const int i = 4 * l + j;
+      if (lora_rank[i] == 0 || !lora_a[i] || !lora_b[i]) continue;
+      GemmLora& lo = e->lora[i];
+      if ((rc = make_gemm_lora(&lo, lora_a[i], lora_b[i], lora_rank[i], rows[j], cols[j]))) {
+        b2e_encoder_destroy(e);
+        return rc;
+      }
+      lo.u_ws = &e->lora_u.p;
+      e->lora_r128 = std::max(e->lora_r128, lo.r128);
+      slots[j]->lora = &lo;
     }
   }
   if ((rc = make_rope_tables(e))) {
@@ -1226,12 +1307,35 @@ int b2e_encoder_create_nf4(const B2EModelDesc* desc, const void* const* weights,
   return create_encoder(desc, weights, n_weights, absmax, device, out);
 }
 
+int b2e_encoder_create_nf4_lora(const B2EModelDesc* desc, const void* const* weights, int n_weights,
+                                const float* const* absmax, int n_absmax, const void* const* lora_a,
+                                const void* const* lora_b, const int* lora_rank, int n_lora, int device,
+                                B2EEncoder** out) {
+  if (!desc || !weights || !absmax || !lora_a || !lora_b || !lora_rank || !out)
+    return fail(B2E_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (n_absmax != 4 * desc->num_layers || n_lora != 4 * desc->num_layers)
+    return fail(B2E_ERR_INVALID, "expected %d NF4 scale pointers and LoRA slots (4 per layer), got %d and %d",
+                4 * desc->num_layers, n_absmax, n_lora);
+  for (int i = 0; i < n_absmax; ++i)
+    if (!absmax[i] || reinterpret_cast<uintptr_t>(absmax[i]) % 16 != 0)
+      return fail(B2E_ERR_INVALID, "NF4 scale pointer %d is null or not 16-byte aligned", i);
+  for (int i = 0; i < n_lora; ++i) {
+    if (lora_rank[i] < 0 || lora_rank[i] % 64 != 0)
+      return fail(B2E_ERR_INVALID, "LoRA slot %d: rank %d must be a non-negative multiple of 64", i, lora_rank[i]);
+    if (lora_rank[i] == 0 || !lora_a[i] || !lora_b[i]) continue;
+    if (reinterpret_cast<uintptr_t>(lora_a[i]) % 16 != 0 || reinterpret_cast<uintptr_t>(lora_b[i]) % 16 != 0)
+      return fail(B2E_ERR_INVALID, "LoRA slot %d: factor pointers must be 16-byte aligned", i);
+  }
+  return create_encoder(desc, weights, n_weights, absmax, device, out, lora_a, lora_b, lora_rank);
+}
+
 void b2e_encoder_destroy(B2EEncoder* e) {
   if (!e) return;
   DeviceGuard guard;
   cudaSetDevice(e->device);
   for (DevBuf<h16>* b : {&e->hidden, &e->qkv, &e->ctx, &e->tmp, &e->ffn}) b->release();
-  e->xres.release(); e->tok_scale.release(); e->stage_in.release(); e->stage_out.release();
+  e->xres.release(); e->tok_scale.release(); e->stage_in.release(); e->stage_out.release(); e->lora_u.release();
   cudaFree(e->rope_cos); cudaFree(e->rope_sin); cudaFree(e->rope_cos2); cudaFree(e->rope_sin2);
   e->pack.release();
   e->drop_graphs();
@@ -1248,6 +1352,7 @@ int64_t b2e_workspace_bytes(const B2EEncoder* e, int B, int S) {
   if (e->has_xres()) bytes += tokens * e->desc.hidden * 4 + (size_t)B * sizeof(float);
   bytes += tokens * sizeof(float) + (size_t)S * sizeof(int) + (size_t)B * (2 * sizeof(int) + sizeof(float));
   bytes += (size_t)B * pool_nsplit(S) * e->desc.hidden * sizeof(float);
+  bytes += tokens * e->lora_r128 * 2;
   return (int64_t)bytes;
 }
 
@@ -1527,7 +1632,7 @@ namespace {
 // b2e_gemm_h16 (absmax null), b2e_gemm_nf4 and b2e_debug_gemm_rows (m_dev set).  An argument the epilogue would not
 // read is an error rather than silently dropped: the gated epilogues add no bias, only B2E_EPI_BIAS_RESID adds resid.
 int gemm_entry(const void* A, const void* W, const float* absmax, const float* bias, const void* resid, void* out,
-               int M, int N, int K, int epi, const int* m_dev, void* stream) {
+               int M, int N, int K, int epi, const int* m_dev, void* stream, const GemmLora* lora = nullptr) {
   if (!A || !W || !out) return fail(B2E_ERR_INVALID, "null tensor pointer");  // bias may be null
   if (absmax && reinterpret_cast<uintptr_t>(absmax) % 16 != 0)
     return fail(B2E_ERR_INVALID, "absmax not 16-byte aligned");
@@ -1544,6 +1649,7 @@ int gemm_entry(const void* A, const void* W, const float* absmax, const float* b
   GemmW tb;
   if ((rc = make_tmap_h16(&ta, A, M, K, 128))) return rc;
   if ((rc = make_gemm_w(&tb, W, absmax, N, K, epi))) return rc;
+  tb.lora = lora;
   return launch_gemm(ta, tb, out, bias, resid, M, N, K, epi, (cudaStream_t)stream, m_dev);
 }
 }  // namespace
@@ -1560,10 +1666,41 @@ int b2e_gemm_nf4(const void* A, const void* codes, const float* absmax, const fl
   return gemm_entry(A, codes, absmax, bias, resid, out, M, N, K, epi, nullptr, stream);
 }
 
+int b2e_gemm_nf4_lora(const void* A, const void* codes, const float* absmax, const void* U, int ldu, const void* Bl,
+                      int R, const float* bias, const void* resid, void* out, int M, int N, int K, int epi,
+                      void* stream) {
+  if (!absmax || !U || !Bl) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (R <= 0 || R % GEMM_BK != 0 || ldu < R)
+    return fail(B2E_ERR_INVALID, "gemm_nf4_lora: need R a positive multiple of 64 and ldu >= R (got %d, %d)", R, ldu);
+  if (reinterpret_cast<uintptr_t>(U) % 16 != 0 || reinterpret_cast<uintptr_t>(Bl) % 16 != 0 || ldu % 8 != 0)
+    return fail(B2E_ERR_INVALID, "gemm_nf4_lora: U and Bl must be 16-byte aligned and ldu a multiple of 8");
+  GemmLora lo;
+  lo.r_blocks = R / GEMM_BK;
+  lo.u = U;
+  lo.ldu = ldu;
+  int rc;
+  if ((rc = check_gemm_shape(M, N, K))) return rc;
+  if ((rc = make_tmap_h16(&lo.tm_b, Bl, N, R, GEMM_BN))) return rc;
+  return gemm_entry(A, codes, absmax, bias, resid, out, M, N, K, epi, nullptr, stream, &lo);
+}
+
 int b2e_debug_gemm_rows(const void* A, const void* W, const float* absmax, const float* bias, const void* resid,
                         void* out, int M, int N, int K, int epi, const int* m_dev, void* stream) {
   if (!m_dev) return fail(B2E_ERR_INVALID, "null m_dev");
   return gemm_entry(A, W, absmax, bias, resid, out, M, N, K, epi, m_dev, stream);
+}
+
+int b2e_debug_gemm_nf4_lora_rows(const void* A, const void* codes, const float* absmax, const void* A_cat,
+                                 const void* B_cat, int R, void* U_ws, const float* bias, const void* resid, void* out,
+                                 int M, int N, int K, int epi, const int* m_dev, void* stream) {
+  if (!absmax || !A_cat || !B_cat || !U_ws || !m_dev) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  int rc;
+  if ((rc = check_gemm_shape(M, N, K))) return rc;
+  GemmLora lo;
+  if ((rc = make_gemm_lora(&lo, A_cat, B_cat, R, N, K))) return rc;
+  h16* ws = static_cast<h16*>(U_ws);
+  lo.u_ws = &ws;
+  return gemm_entry(A, codes, absmax, bias, resid, out, M, N, K, epi, m_dev, stream, &lo);
 }
 
 int b2e_attention_d64(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,

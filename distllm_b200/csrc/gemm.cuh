@@ -30,6 +30,11 @@
 // into shared memory by the producer warpgroup from 4-bit codes and fp32 block scales (gemm_nf4_producer) instead of
 // being loaded by the TMA; consumers, hand-over, tile walk and epilogues are the same code.
 //
+// gemm_nf4_lora_kernel (a LoRA adapter kept unmerged beside NF4 weights) is the NF4 body with R/64 more k-blocks
+// per tile: U = X . A_cat^T and B_cat, both 16-bit, TMA-loaded into the stage as the 16-bit kernel loads A and W, so
+// y = epi(X . dequant(W)^T + U . B_cat^T + bias): every epilogue applies to the sum, as peft's layer adds the
+// low-rank term before the activation.
+//
 // This replaces the cuBLAS nn.Linear calls HF BERT issues from
 // transformers/models/bert/modeling_bert.py:180-182 (q,k,v), :294-298 (attn out), :339-342 (FFN up +
 // GELU), :352-356 (FFN down), reached from distllm/embed/encoders/auto.py:135.
@@ -206,9 +211,19 @@ __device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t
 // the loads: the A box of each k-block once its stage is free, and the code box + scales of the k-block
 // GEMM_NF4_RAW ahead into the raw slot the warpgroup has just finished reading.  A stage's full barrier completes
 // on the A bytes plus thread 0's arrival after the warpgroup's named-barrier sync.
+//
+// LORA: each tile's K/64 NF4 k-blocks are followed by r_blocks tail k-blocks of the low-rank term U . B_cat^T
+// (U = X . A_cat^T, 16-bit [M, R]; B_cat 16-bit [N, R], the scaling folded in).  A tail stage is two TMA loads in
+// the 16-bit GEMM's layout -- U at (64 r, m0) into the A region, B_cat at (64 r, n0) into the W region -- and
+// thread 0 completes its full barrier with the expect_tx of the whole stage and its second arrival.  No
+// dequantisation, no proxy fence, no named-barrier sync; the raw ring counts base k-blocks only.  All 128 threads
+// still wait for each tail stage to be free, so that none of them is ever more than one stage ahead of the ring.
+template <bool LORA = false>
 __device__ __forceinline__ void gemm_nf4_producer(const CUtensorMap* tm_a, const CUtensorMap* tm_codes,
                                                   const float* __restrict__ absmax, const GemmTiles& tl, int N,
-                                                  int kblocks, uint32_t sb, uint32_t full_bar, uint32_t empty_bar) {
+                                                  int kblocks, uint32_t sb, uint32_t full_bar, uint32_t empty_bar,
+                                                  const CUtensorMap* tm_u = nullptr,
+                                                  const CUtensorMap* tm_bl = nullptr, int r_blocks = 0) {
   using P = GemmPlan<true>;
   const int p = static_cast<int>(threadIdx.x) - 256;
   const uint32_t raw0 = sb + P::RAW_OFFSET;
@@ -230,6 +245,10 @@ __device__ __forceinline__ void gemm_nf4_producer(const CUtensorMap* tm_a, const
   if (p == 0) {
     tma_prefetch_desc(tm_a);
     tma_prefetch_desc(tm_codes);
+    if constexpr (LORA) {
+      tma_prefetch_desc(tm_u);
+      tma_prefetch_desc(tm_bl);
+    }
     while (ld < total && ld < GEMM_NF4_RAW) load_raw();
   }
   int stage = 0, slot = 0;
@@ -274,20 +293,39 @@ __device__ __forceinline__ void gemm_nf4_producer(const CUtensorMap* tm_a, const
       if (++stage == P::STAGES) { stage = 0; phase ^= 1u; }
       if (++slot == GEMM_NF4_RAW) { slot = 0; raw_phase ^= 1u; }
     }
+    if constexpr (LORA) {
+      const int n0 = ((tl.first + i * tl.stride) % tl.n_tiles) * GEMM_BN;
+      for (int r = 0; r < r_blocks; ++r) {
+        // every producer thread waits, although only thread 0 loads: a thread that skipped these waits would reach
+        // the next tile's NF4 stages up to r_blocks positions ahead, and from STAGES positions on its parity wait
+        // could pass on a phase that completed a whole ring earlier
+        mbar_wait(empty_bar + 8u * stage, phase ^ 1u);
+        if (p == 0) {
+          const uint32_t dst = sb + stage * GEMM_STAGE_BYTES;
+          const uint32_t fb = full_bar + 8u * stage;
+          mbar_expect_tx(fb, GEMM_STAGE_BYTES);
+          tma_load_2d(dst, tm_u, fb, r * GEMM_BK, m0);
+          tma_load_2d(dst + GEMM_A_BYTES, tm_bl, fb, r * GEMM_BK, n0);
+          mbar_arrive(fb);
+        }
+        if (++stage == P::STAGES) { stage = 0; phase ^= 1u; }
+      }
+    }
   }
 }
 
-// NF4 = false: W is a 16-bit [N,K] map.  NF4 = true: tm_b is the uint8 code map [N,K/2] (box 32 x 128) and absmax
-// the block scales [K/64, N] (gemm_nf4_producer).
-template <int EPI, bool TL = false, bool NF4 = false, int BN = GEMM_BN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
-                      const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x BN
-                      const __grid_constant__ CUtensorMap tm_out,  // out [M,N] (GLU: [M,N/2]) box 64 x 128
-                      h16* __restrict__ out, const float* __restrict__ bias, const h16* __restrict__ resid,
-                      int M, int N, int K, const int* __restrict__ m_dev, const float* __restrict__ absmax) {
+// The kernel body: gemm_h16_wgmma_kernel, and (LORA) gemm_nf4_lora_kernel.  NF4 = false: W is a 16-bit [N,K] map.
+// NF4 = true: tm_b is the uint8 code map [N,K/2] (box 32 x 128) and absmax the block scales [K/64, N]
+// (gemm_nf4_producer).  LORA: the consumers run K/64 + r_blocks k-blocks per tile, the tail ones over U and B_cat.
+template <int EPI, bool TL, bool NF4, int BN, bool LORA>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const CUtensorMap& tm_out,
+                                          h16* __restrict__ out, const float* __restrict__ bias,
+                                          const h16* __restrict__ resid, int M, int N, int K,
+                                          const int* __restrict__ m_dev, const float* __restrict__ absmax,
+                                          const CUtensorMap* tm_u, const CUtensorMap* tm_bl, int r_blocks) {
   using P = GemmPlan<NF4, BN>;
   static_assert(!epi_is_glu(EPI) || BN == 128, "the gated epilogues pair gate and up within a 128-row W tile");
+  static_assert(!LORA || (NF4 && !TL), "the low-rank tail rides on the NF4 producer");
   if (m_dev != nullptr) M = __ldg(m_dev);   // device-resident row count (packed token layout)
   const GemmTiles tl = gemm_tiles<BN>(M, N);
   extern __shared__ uint8_t smem_raw[];
@@ -296,6 +334,7 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   const uint32_t empty_bar = full_bar + 8u * P::STAGES;
   const int warp = threadIdx.x >> 5;
   const int kblocks = K / GEMM_BK;
+  const int kb_tile = LORA ? kblocks + r_blocks : kblocks;   // the k-blocks of one tile in the ring
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < P::STAGES; ++s) {
@@ -314,7 +353,7 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
   if (warp >= 8) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(P::PRODUCER_REGS));
     if constexpr (NF4) {
-      gemm_nf4_producer(&tm_a, &tm_b, absmax, tl, N, kblocks, sb, full_bar, empty_bar);
+      gemm_nf4_producer<LORA>(&tm_a, &tm_b, absmax, tl, N, kblocks, sb, full_bar, empty_bar, tm_u, tm_bl, r_blocks);
     } else if (warp == 8 && elect_one()) {
       tma_prefetch_desc(&tm_a);
       tma_prefetch_desc(&tm_b);
@@ -368,12 +407,12 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
 #pragma unroll
     for (int x = 0; x < BN / 2; ++x) acc[0][x] = acc[1][x] = 0.0f;
     if (i > 0) named_bar_sync(GEMM_BAR_TURN + wg, 256);
-    // this tile's k-blocks follow the i * kblocks ones of the earlier turns in the ring
-    const int it = i * kblocks;
+    // this tile's k-blocks follow the i * kb_tile ones of the earlier turns in the ring
+    const int it = i * kb_tile;
     int stage = it % P::STAGES;
     uint32_t phase = (it / P::STAGES) & 1u;
     int prev = -1;
-    for (int kb = 0; kb < kblocks; ++kb) {
+    for (int kb = 0; kb < kb_tile; ++kb) {
       mbar_wait(full_bar + 8u * stage, phase);
       const uint32_t a_addr = sb + stage * P::STAGE_BYTES;
       const uint64_t a0 = make_smem_desc_sw128(a_addr), a1 = make_smem_desc_sw128(a_addr + 64 * 128);
@@ -512,6 +551,32 @@ gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 
     if (TL && clk != nullptr && wg == 0 && t == 0 && i / 2 < 256) clk[768 + i / 2] = clock64();
   }
   if (t == 0) tma_store_wait_all();   // the stores have read shared memory before the CTA leaves
+}
+
+template <int EPI, bool TL = false, bool NF4 = false, int BN = GEMM_BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_h16_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a,    // [M,K] box 64 x 128
+                      const __grid_constant__ CUtensorMap tm_b,    // [N,K] box 64 x BN
+                      const __grid_constant__ CUtensorMap tm_out,  // out [M,N] (GLU: [M,N/2]) box 64 x 128
+                      h16* __restrict__ out, const float* __restrict__ bias, const h16* __restrict__ resid,
+                      int M, int N, int K, const int* __restrict__ m_dev, const float* __restrict__ absmax) {
+  gemm_body<EPI, TL, NF4, BN, false>(tm_a, tm_b, tm_out, out, bias, resid, M, N, K, m_dev, absmax, nullptr, nullptr, 0);
+}
+
+// y = epi(A . dequant(W)^T + U . B_cat^T + bias [+ resid]): the NF4 GEMM with r_blocks = R/64 extra k-blocks per
+// tile.  Each output sums the same products in the same order as the 16-bit GEMM over the K-concatenated operands
+// [A | U] and [round16(dequant(W)) | B_cat].
+template <int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_nf4_lora_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                     const __grid_constant__ CUtensorMap tm_out, h16* __restrict__ out,
+                     const float* __restrict__ bias, const h16* __restrict__ resid, int M, int N, int K,
+                     const int* __restrict__ m_dev, const float* __restrict__ absmax,
+                     const __grid_constant__ CUtensorMap tm_u,    // U [M, >= R] box 64 x 128
+                     const __grid_constant__ CUtensorMap tm_bl,   // B_cat [N, R] box 64 x 128
+                     int r_blocks) {
+  gemm_body<EPI, false, true, GEMM_BN, true>(tm_a, tm_b, tm_out, out, bias, resid, M, N, K, m_dev, absmax, &tm_u,
+                                             &tm_bl, r_blocks);
 }
 
 }  // namespace b2e

@@ -46,8 +46,13 @@ class AutoEncoderConfig(BaseConfig):
     eval_mode: bool = True
     # Kept for compatibility: there is no tracing compiler in this path
     compile_model: bool = False
+    # The model id may name a PEFT adapter checkpoint (adapter_config.json without config.json, LoRA or IA3): the
+    # base model is its base_model_name_or_path, and the tokenizer tokenizer_name, else the adapter directory if it
+    # holds tokenizer files, else the base (embed/encoders/adapters.py).
     # NF4 (bitsandbytes) weight quantisation: every transformer-block weight matrix is held on the device in 4-bit
-    # NF4 (3.56x less memory than 16 bits) and dequantised inside the GEMMs to exactly dequant(quant(W))
+    # NF4 (3.56x less memory than 16 bits) and dequantised inside the GEMMs to exactly dequant(quant(W)).  A LoRA
+    # adapter stays unmerged next to the NF4 weights; an IA3 adapter is merged into dequant(quant(W)) at load time,
+    # in 16 bits, as with nf4_storage: False
     quantization: bool = True
     # With quantization: False dequantises once at load time into 16-bit matrices instead -- the same results bit for
     # bit, 3.56x the weight memory, and the faster 16-bit GEMM (README: the NF4 GEMM runs at 0.64-0.78x of it)
@@ -68,22 +73,29 @@ class AutoEncoder:
         from transformers import AutoModel
         from transformers import AutoTokenizer
 
-        hf_config = AutoConfig.from_pretrained(config.pretrained_model_name_or_path)
+        from distllm_b200.embed.encoders import adapters
+
+        # a PEFT adapter checkpoint (adapter_config.json, no config.json) runs on its base_model_name_or_path
+        base_path, adapter_dir = adapters.resolve(config.pretrained_model_name_or_path)
+        hf_config = AutoConfig.from_pretrained(base_path)
         if hf_config.model_type not in _SUPPORTED_MODEL_TYPES:
             raise NotImplementedError(
                 f'model_type={hf_config.model_type!r} has no native sm_90a forward pass yet '
                 f'(built: {_SUPPORTED_MODEL_TYPES}); there is no eager fallback.',
             )
         _NATIVE_BY_MODEL_TYPE[hf_config.model_type].validate(hf_config)   # before any weight is loaded
-        model = AutoModel.from_pretrained(config.pretrained_model_name_or_path)
+        model = AutoModel.from_pretrained(base_path)
         tokenizer = AutoTokenizer.from_pretrained(
-            config.tokenizer_name or config.pretrained_model_name_or_path,
+            adapters.tokenizer_source(config.tokenizer_name, config.pretrained_model_name_or_path, base_path),
         )
         # proper truncation, as auto.py:74
         tokenizer.model_max_length = hf_config.max_position_embeddings
 
         self.config = config
         state_dict = model.state_dict()
+        adapter = adapters.load_adapter(adapter_dir, state_dict) if adapter_dir is not None else None
+        # modules whose adapter tensors were ignored (heads downstream of the last hidden state)
+        self.adapter_ignored = list(adapter.ignored) if adapter is not None else []
         nf4 = False
         if config.quantization:
             # the reference's default (auto.py:44-56): every nn.Linear weight goes through 4-bit NormalFloat with
@@ -92,16 +104,25 @@ class AutoEncoder:
             # in NF4 on the device, quantised one matrix at a time, and the GEMMs dequantise them exactly.  A
             # checkpoint whose quantised matrices are not all in 64-column blocks (no published checkpoint of a built
             # family), or a config with nf4_storage: False, gets dequant(quant(W)) computed here once, in 16 bits: the
-            # same results, without the saving.
+            # same results, without the saving.  A LoRA adapter stays outside the quantisation, as in the reference
+            # (dequant(NF4(W)) x + s B A x): under NF4 storage the GEMMs add it unmerged, otherwise it is merged in
+            # fp32 into dequant(quant(W)).  An IA3 adapter always takes the second path.
             from distllm_b200.embed.encoders.nf4 import is_quantized_linear
             from distllm_b200.embed.encoders.nf4 import nf4_storable
             from distllm_b200.embed.encoders.nf4 import quantize_state_dict_nf4
 
-            nf4 = config.nf4_storage and all(nf4_storable(t) for name, t in state_dict.items()
-                                             if is_quantized_linear(name, t))
+            nf4 = (config.nf4_storage and (adapter is None or adapter.peft_type == 'LORA')
+                   and all(nf4_storable(t) for name, t in state_dict.items() if is_quantized_linear(name, t)))
             if not nf4:
                 state_dict = quantize_state_dict_nf4(state_dict, device='cuda' if torch.cuda.is_available() else None)
-        self._native = _NATIVE_BY_MODEL_TYPE[hf_config.model_type](hf_config, state_dict, nf4=nf4)
+        lora = None
+        if adapter is not None:
+            if nf4:
+                lora = adapter.lora
+            else:
+                state_dict = adapters.merge_adapter(state_dict, adapter)
+        extra = {'lora': lora} if lora else {}   # without an adapter the encoder is built exactly as before
+        self._native = _NATIVE_BY_MODEL_TYPE[hf_config.model_type](hf_config, state_dict, nf4=nf4, **extra)
         del model, state_dict
         self._tokenizer = tokenizer
         self._dtype = torch.float16 if config.half_precision else torch.float32
@@ -112,6 +133,7 @@ class AutoEncoder:
         """Wrap an already-built native encoder (synthetic weights, tests, benchmarks)."""
         self = cls.__new__(cls)
         self.config = None
+        self.adapter_ignored = []
         self._native = native
         self._tokenizer = tokenizer
         self._dtype = torch.float16 if half_precision else torch.float32

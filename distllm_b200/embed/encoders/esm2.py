@@ -48,20 +48,30 @@ class Esm2Encoder:
         from transformers import EsmForMaskedLM
         from transformers import EsmTokenizer
 
-        hf_config = AutoConfig.from_pretrained(config.pretrained_model_name_or_path)
+        from distllm_b200.embed.encoders import adapters
+
+        # a PEFT adapter checkpoint runs on its base_model_name_or_path, merged into the 16-bit weights
+        base_path, adapter_dir = adapters.resolve(config.pretrained_model_name_or_path)
+        hf_config = AutoConfig.from_pretrained(base_path)
         if hf_config.model_type != 'esm':
             raise NotImplementedError(f'model_type={hf_config.model_type!r} is not an ESM checkpoint')
         NativeEsm2Encoder.validate(hf_config)   # unsupported shapes fail here, before the weights load
-        model = EsmForMaskedLM.from_pretrained(config.pretrained_model_name_or_path)
+        model = EsmForMaskedLM.from_pretrained(base_path)
         tokenizer = EsmTokenizer.from_pretrained(
-            config.tokenizer_path or config.pretrained_model_name_or_path,
+            adapters.tokenizer_source(config.tokenizer_path, config.pretrained_model_name_or_path, base_path),
         )
         # proper truncation, as esm2.py:66
         tokenizer.model_max_length = hf_config.max_position_embeddings
 
         self.config = config
-        self._native = NativeEsm2Encoder(hf_config, model.state_dict())
-        del model
+        state_dict = model.state_dict()
+        self.adapter_ignored = []
+        if adapter_dir is not None:
+            adapter = adapters.load_adapter(adapter_dir, state_dict)
+            self.adapter_ignored = list(adapter.ignored)
+            state_dict = adapters.merge_adapter(state_dict, adapter)
+        self._native = NativeEsm2Encoder(hf_config, state_dict)
+        del model, state_dict
         self._tokenizer = tokenizer
         self._dtype = torch.float16 if config.half_precision else torch.float32
 
@@ -71,6 +81,7 @@ class Esm2Encoder:
         """Wrap an already-built native encoder (synthetic weights, tests, benchmarks)."""
         self = cls.__new__(cls)
         self.config = None
+        self.adapter_ignored = []
         self._native = native
         self._tokenizer = tokenizer
         self._dtype = torch.float16 if half_precision else torch.float32

@@ -24,12 +24,18 @@ class NativeBertEncoder:
     _ARCH = 'bert'    # picks the build of the library (16-bit storage type): _native.storage_for_arch
 
     def __init__(self, hf_config, state_dict: Mapping[str, torch.Tensor],
-                 device: torch.device | str | None = None, storage: str | None = None, nf4: bool = False) -> None:
+                 device: torch.device | str | None = None, storage: str | None = None, nf4: bool = False,
+                 lora: Mapping[str, tuple[torch.Tensor, torch.Tensor, float]] | None = None) -> None:
         """``nf4``: hold every weight matrix in 4-bit NF4 (``b2e_encoder_create_nf4``), quantised from
         ``state_dict`` one checkpoint matrix at a time on the device; the results equal bit for bit those of the
-        16-bit encoder built from ``nf4.quantize_state_dict_nf4(state_dict)``."""
+        16-bit encoder built from ``nf4.quantize_state_dict_nf4(state_dict)``.
+
+        ``lora`` (NF4 only; ``adapters.Adapter.lora``): LoRA modules kept unmerged, added by the NF4 GEMMs as extra
+        k-blocks (``b2e_encoder_create_nf4_lora``, ``weights.lora_slot_factors``)."""
         if nf4 and self._ARCH == 'esm':
             raise NotImplementedError('ESM-2 has no quantised configuration')
+        if lora and not nf4:
+            raise ValueError('unmerged LoRA needs NF4 storage; merge the adapter into 16-bit weights instead')
         self.storage = storage or _native.storage_for_arch(self._ARCH)
         lib = _native.load(self.storage)
         if not torch.cuda.is_available():
@@ -55,10 +61,22 @@ class NativeBertEncoder:
             raise _native.NativeError(f'weight list has {n} tensors, ABI expects {expected}')
         ptrs = (C.c_void_p * n)(*[(t.codes if isinstance(t, W.Nf4Matrix) else t).data_ptr() for t in self._weights])
         handle = C.c_void_p()
+        self._lora = (W.lora_slot_factors(self._ARCH, hf_config, lora, self.device,
+                                          _native.STORAGE_TORCH_DTYPE[self.storage]) if lora else [])
         if nf4:
             scales = [t.absmax.data_ptr() for t in self._weights if isinstance(t, W.Nf4Matrix)]
-            _native.check(lib.b2e_encoder_create_nf4(C.byref(self.desc), ptrs, n, (C.c_void_p * len(scales))(*scales),
-                                                     len(scales), self.device.index, C.byref(handle)), lib)
+            scale_ptrs = (C.c_void_p * len(scales))(*scales)
+            if self._lora:
+                k = len(self._lora)
+                a_ptrs = (C.c_void_p * k)(*[f[0].data_ptr() if f else None for f in self._lora])
+                b_ptrs = (C.c_void_p * k)(*[f[1].data_ptr() if f else None for f in self._lora])
+                ranks = (C.c_int * k)(*[f[2] if f else 0 for f in self._lora])
+                _native.check(lib.b2e_encoder_create_nf4_lora(
+                    C.byref(self.desc), ptrs, n, scale_ptrs, len(scales), a_ptrs, b_ptrs, ranks, k,
+                    self.device.index, C.byref(handle)), lib)
+            else:
+                _native.check(lib.b2e_encoder_create_nf4(C.byref(self.desc), ptrs, n, scale_ptrs, len(scales),
+                                                         self.device.index, C.byref(handle)), lib)
         else:
             _native.check(lib.b2e_encoder_create(C.byref(self.desc), ptrs, n, self.device.index,
                                                  C.byref(handle)), lib)
@@ -102,6 +120,10 @@ class NativeBertEncoder:
     def weight_bytes(self) -> dict[str, int]:
         """Device bytes of the weights: ``matrix`` (16-bit matrices, or NF4 codes + scales) and ``other``."""
         return W.device_weight_bytes(self._weights)
+
+    def lora_bytes(self) -> int:
+        """Device bytes of the unmerged LoRA factors (A_cat and B_cat of every adapted slot)."""
+        return sum(f[0].nbytes + f[1].nbytes for f in self._lora if f)
 
     def workspace_bytes(self, batch: int, seq: int) -> int:
         return int(self._lib.b2e_workspace_bytes(self._handle, batch, seq))

@@ -666,3 +666,90 @@ def random_modernbert_state_dict(hf_config, seed: int = 0, device: torch.device 
         sd[p + 'mlp.Wi.weight'] = normal(2 * i, h)
         sd[p + 'mlp.Wo.weight'] = normal(h, i)
     return sd
+
+
+# ------------------------------------------------------------------------------ LoRA under NF4 storage
+# ``b2e_encoder_create_nf4_lora`` takes per GEMM slot (4 per layer, the absmax order: Wqkv, Wo, W1, W2) the factors of
+# the slot's low-rank term, delta(slot) = B_cat . A_cat:
+#
+#   A_cat  16-bit [round_up(R, 128), K]: the A rows of the slot's adapted modules stacked (Q | K | V, gate | up), zero
+#          rows below; ModernBERT's mlp.Wo gets the zero columns of its padded K
+#   B_cat  16-bit [N, round_up(R, 64)]: module i's s_i B_i in the rows of its outputs and the columns of its A rows
+#          (s folded in fp32 before the storage rounding), then the slot's row layout -- Q | K | V, the gate/up
+#          interleave of interleave_gate_up, ModernBERT's padded Wi halves -- and zero columns on the right
+#
+# so that the NF4 GEMM's tail k-blocks add U . B_cat^T with U = X . A_cat^T, R = the sum of the modules' ranks.
+
+
+def _lora_slots(arch: str, hf_config, layer: int) -> list[tuple[list[tuple[str, int]], int, str]]:
+    """The four GEMM slots of ``layer``: ([(module, output rows)], K, row layout)."""
+    h = hf_config.hidden_size
+    if arch == 'bert':
+        p, i = f'encoder.layer.{layer}.', hf_config.intermediate_size
+        return [([(p + f'attention.self.{n}', h) for n in ('query', 'key', 'value')], h, 'cat'),
+                ([(p + 'attention.output.dense', h)], h, 'cat'),
+                ([(p + 'intermediate.dense', i)], h, 'cat'),
+                ([(p + 'output.dense', h)], i, 'cat')]
+    if arch in ('mistral', 'qwen3'):
+        p, i = f'layers.{layer}.', hf_config.intermediate_size
+        heads, kv = hf_config.num_attention_heads, hf_config.num_key_value_heads
+        d = getattr(hf_config, 'head_dim', None) or h // heads
+        return [([(p + 'self_attn.q_proj', heads * d), (p + 'self_attn.k_proj', kv * d),
+                  (p + 'self_attn.v_proj', kv * d)], h, 'cat'),
+                ([(p + 'self_attn.o_proj', h)], heads * d, 'cat'),
+                ([(p + 'mlp.gate_proj', i), (p + 'mlp.up_proj', i)], h, 'gate_up'),
+                ([(p + 'mlp.down_proj', h)], i, 'cat')]
+    if arch == 'modernbert':
+        p, i = f'layers.{layer}.', hf_config.intermediate_size
+        return [([(p + 'attn.Wqkv', 3 * h)], h, 'cat'),
+                ([(p + 'attn.Wo', h)], h, 'cat'),
+                ([(p + 'mlp.Wi', 2 * i)], h, 'geglu'),
+                ([(p + 'mlp.Wo', h)], i, 'pad_k')]
+    raise NotImplementedError(f'{arch}: no quantised configuration, so no unmerged LoRA path')
+
+
+_MODEL_PREFIX = {'bert': 'bert.', 'mistral': 'model.', 'qwen3': 'model.', 'modernbert': 'model.'}
+
+
+def lora_slot_factors(arch: str, hf_config, lora: Mapping[str, tuple[torch.Tensor, torch.Tensor, float]],
+                      device: torch.device, dtype: torch.dtype) -> list[tuple[torch.Tensor, torch.Tensor, int] | None]:
+    """LoRA modules ``{module: (A [r, in], B [out, r], s)}`` (state-dict names) -> per slot (A_cat, B_cat, R) with
+    R = round_up(sum of ranks, 64), or None for a slot without an adapter; in ``dtype`` on ``device``."""
+    pre = _MODEL_PREFIX[arch]
+    lo = {k[len(pre):] if k.startswith(pre) else k: v for k, v in lora.items()}
+    used = set()
+    out: list = []
+    for layer in range(hf_config.num_hidden_layers):
+        for modules, k, layout in _lora_slots(arch, hf_config, layer):
+            present = [(m, rows) for m, rows in modules if m in lo]
+            if not present:
+                out.append(None)
+                continue
+            used.update(m for m, _ in present)
+            r = sum(lo[m][0].shape[0] for m, _ in present)
+            r64, r128 = (r + 63) // 64 * 64, (r + 127) // 128 * 128
+            a_cat = torch.zeros((r128, k), dtype=torch.float32, device=device)
+            b_full = torch.zeros((sum(rows for _, rows in modules), r64), dtype=torch.float32, device=device)
+            row = col = 0
+            for m, rows in modules:
+                if m in lo:
+                    a, b, s = lo[m]
+                    ri = a.shape[0]
+                    a_cat[col:col + ri] = a.to(device=device, dtype=torch.float32)
+                    b_full[row:row + rows, col:col + ri] = s * b.to(device=device, dtype=torch.float32)
+                    col += ri
+                row += rows
+            if layout == 'gate_up':
+                half = b_full.shape[0] // 2
+                b_full = interleave_gate_up(b_full[:half], b_full[half:])
+            elif layout == 'geglu':
+                half = b_full.shape[0] // 2
+                pad = modernbert_padded_intermediate(half) - half
+                b_full = interleave_gate_up(pad_rows(b_full[:half], pad), pad_rows(b_full[half:], pad))
+            elif layout == 'pad_k':
+                a_cat = pad_cols(a_cat, modernbert_padded_intermediate(k) - k)
+            out.append((to_storage(a_cat, device, dtype), to_storage(b_full, device, dtype), r64))
+    missing = sorted(set(lo) - used)
+    if missing:
+        raise ValueError(f'LoRA modules outside the GEMM slots of {arch}: {missing[:8]}')
+    return out

@@ -129,6 +129,17 @@ int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int
  * bit for bit those of b2e_encoder_create on the dequantised 16-bit matrices. */
 int b2e_encoder_create_nf4(const B2EModelDesc* desc, const void* const* weights, int n_weights,
                            const float* const* absmax, int n_absmax, int device, B2EEncoder** out);
+/* b2e_encoder_create_nf4 with LoRA adapters kept unmerged (distllm_b200/embed/encoders/adapters.py): the layer
+ * computes dequant(W) x + B_cat (A_cat x), the adapter outside the quantisation, as peft's LoRA layer does on a
+ * 4-bit base.  lora_a / lora_b / lora_rank hold n_lora = 4 * num_layers entries in the absmax order; entry i is
+ * R = lora_rank[i] (a multiple of 64; 0 or a NULL factor: no adapter on that slot), A_cat 16-bit
+ * [round_up(R, 128), K] and B_cat 16-bit [N, R] with the scaling folded in (weights.py: lora_slot_factors), both
+ * 16-byte aligned.  Each such GEMM first computes U = X . A_cat^T into a workspace [tokens, max round_up(R, 128)]
+ * and then runs R / 64 extra k-blocks of U . B_cat^T inside the NF4 GEMM, before the epilogue. */
+int b2e_encoder_create_nf4_lora(const B2EModelDesc* desc, const void* const* weights, int n_weights,
+                                const float* const* absmax, int n_absmax, const void* const* lora_a,
+                                const void* const* lora_b, const int* lora_rank, int n_lora, int device,
+                                B2EEncoder** out);
 void b2e_encoder_destroy(B2EEncoder* enc);
 
 /* Bytes of device workspace the handle holds for a [B,S] batch (grown lazily, never shrunk). */
@@ -175,6 +186,12 @@ int b2e_gemm_h16(const void* A, const void* W, const float* bias, const void* re
 /* The same with W in NF4: codes uint8 [N, K/2] and fp32 scales absmax [K/64, N] (see b2e_encoder_create_nf4). */
 int b2e_gemm_nf4(const void* A, const void* codes, const float* absmax, const float* bias, const void* resid,
                  void* out, int M, int N, int K, int epilogue, void* stream);
+/* b2e_gemm_nf4 plus a low-rank term: out = epi(A . dequant(W)^T + U[:, :R] . Bl^T + bias [+ resid]), U [M, ldu]
+ * (ldu >= R, a multiple of 8), Bl [N, R], R a multiple of 64.  Equal bit for bit to b2e_gemm_h16 on the
+ * K-concatenated operands [A | U[:, :R]] and [dequant(W) | Bl]. */
+int b2e_gemm_nf4_lora(const void* A, const void* codes, const float* absmax, const void* U, int ldu, const void* Bl,
+                      int R, const float* bias, const void* resid, void* out, int M, int N, int K, int epilogue,
+                      void* stream);
 /* qkv [B*S, 3*heads*64] -> ctx [B*S, heads*64]; `reserved` must be NULL (it was a debug score dump). */
 int b2e_attention_d64(const void* qkv, const int64_t* attention_mask, void* ctx, int B, int S,
                       int heads, float* reserved, void* stream);

@@ -39,6 +39,12 @@ int b2e_debug_gemm_bn(int n, int epi, int nf4, int* out);
  * written.  M sizes the grid and the tensor maps. */
 int b2e_debug_gemm_rows(const void* A, const void* W, const float* absmax, const float* bias, const void* resid,
                         void* out, int M, int N, int K, int epi, const int* m_dev, void* stream);
+/* b2e_gemm_nf4_lora as an NF4 + LoRA encoder slot runs it, with the device row count *m_dev (as above): U = A . A_cat^T
+ * on the 16-bit GEMM into U_ws [M, round_up(R, 128)] (A_cat 16-bit [round_up(R, 128), K]), then the NF4 GEMM with
+ * R / 64 tail k-blocks over U and B_cat [N, R].  Rows from *m_dev to M of out are not written. */
+int b2e_debug_gemm_nf4_lora_rows(const void* A, const void* codes, const float* absmax, const void* A_cat,
+                                 const void* B_cat, int R, void* U_ws, const float* bias, const void* resid, void* out,
+                                 int M, int N, int K, int epi, const int* m_dev, void* stream);
 /* 0: keep the padded [B, S] token layout on every path; 1 (default, also B2E_PACKED=1): pooled forward passes run
  * on the attended tokens only (csrc/pack.cuh).  Drops the handle's cached CUDA graphs' validity: call it before
  * b2e_embed_host, not between its batches. */
