@@ -99,6 +99,8 @@ DEBUG_EXPORTS = (
     'b2e_debug_topk_tc_fell_back',
     'b2e_debug_attention_packed',
     'b2e_debug_rotary',
+    'b2e_debug_embed',
+    'b2e_debug_norm',
 )
 
 
@@ -440,6 +442,52 @@ def debug_rotary_(enc, layer: int, qkv: torch.Tensor, attention_mask: torch.Tens
         check(lib.b2e_debug_rotary(enc._handle, layer, qkv.data_ptr(), attention_mask.data_ptr(), b, s,
                                    stream_ptr(qkv.device)), lib)
     return qkv
+
+
+def debug_embed(enc, input_ids: torch.Tensor, attention_mask: torch.Tensor,
+                token_type_ids: torch.Tensor | None = None) -> tuple[torch.Tensor | None, torch.Tensor | None]:
+    """Debug hook: the embedding step of encoder ``enc`` (embed.encoders.native) in the token layout it derives from
+    ``attention_mask`` (see attention_packed): (16-bit rows [B*S, H] or None, fp32 residual stream [B*S, H] or None),
+    as the family writes them (BERT the first, ESM-2 / Mistral / Qwen3 the second, ModernBERT both).  Rows the step
+    does not write are zero."""
+    lib = enc._lib
+    for t, what in ((input_ids, 'input_ids'), (attention_mask, 'attention_mask'), (token_type_ids, 'token_type_ids')):
+        if t is not None and (_cuda_contig(t, what).dtype != torch.int64 or t.shape != input_ids.shape):
+            raise NativeError(f'{what} must be int64 [B, S]')
+    b, s = input_ids.shape
+    arch, h = enc.desc.arch, enc.desc.hidden
+    out16 = (torch.zeros((b * s, h), dtype=STORAGE_TORCH_DTYPE[enc.storage], device=input_ids.device)
+             if arch in (ARCH_BERT, ARCH_MODERNBERT) else None)
+    xres = torch.zeros((b * s, h), dtype=torch.float32, device=input_ids.device) if arch != ARCH_BERT else None
+    lib.b2e_debug_embed.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int] + [C.c_void_p] * 3
+    with torch.cuda.device(input_ids.device):
+        check(lib.b2e_debug_embed(enc._handle, input_ids.data_ptr(), attention_mask.data_ptr(), _ptr(token_type_ids),
+                                  b, s, _ptr(out16), _ptr(xres), stream_ptr(input_ids.device)), lib)
+    return out16, xres
+
+
+NORM_POST_LN, NORM_ADD_LN, NORM_ADD_RMS = 0, 1, 2   # b2e_debug_norm's kinds
+
+
+def debug_norm(kind: int, xres: torch.Tensor | None, add: torch.Tensor | None, resid: torch.Tensor | None,
+               gamma: torch.Tensor, beta: torch.Tensor | None, eps: float, out_dtype: torch.dtype) -> torch.Tensor:
+    """Debug hook: one norm step of the trunks with the caller's gains.  ``NORM_POST_LN``: LayerNorm(add + resid) of
+    16-bit rows; ``NORM_ADD_LN`` / ``NORM_ADD_RMS``: ``xres += add`` in place (fp32; ``add`` may be None), then
+    LayerNorm / RMSNorm of xres.  Returns [rows, H] in ``out_dtype`` (float32 or the 16-bit storage type)."""
+    x = add if kind == NORM_POST_LN else xres
+    for t, what in ((xres, 'xres'), (add, 'add'), (resid, 'resid'), (gamma, 'gamma'), (beta, 'beta')):
+        if t is not None:
+            _cuda_contig(t, what)
+    storage = storage_of(add.dtype) if add is not None else storage_of(out_dtype)
+    lib = load(storage)
+    rows, h = x.shape
+    out = torch.empty((rows, h), dtype=out_dtype, device=x.device)
+    lib.b2e_debug_norm.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int, C.c_float,
+                                                                         C.c_void_p, C.c_void_p]
+    with torch.cuda.device(x.device):
+        check(lib.b2e_debug_norm(kind, h, _ptr(xres), _ptr(add), _ptr(resid), gamma.data_ptr(), _ptr(beta),
+                                 out.data_ptr(), dtype_code(out_dtype), rows, eps, None, stream_ptr(x.device)), lib)
+    return out
 
 
 def qk_norm_rope_(qkv: torch.Tensor, q_gamma: torch.Tensor, k_gamma: torch.Tensor, cos: torch.Tensor,

@@ -846,6 +846,41 @@ void launch_rotary(B2EEncoder* e, int l, h16* qkv, int M, int S, cudaStream_t st
         qkv, cos_t, sin_t, M, S, 2 * d.heads, 3 * d.hidden, lay.t_real, lay.tok_src);
 }
 
+// The embedding step of a family over M = B*S rows in the token layout `lay`: BERT embed_layernorm into hidden, ESM-2
+// the token-dropout scales (into e->tok_scale) and esm_embed into xres, Mistral / Qwen3 the gather into xres,
+// ModernBERT the gather into xres and its LayerNorm into hidden.  The trunks and b2e_debug_embed launch it.
+int launch_embed(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t* types, int B, int S,
+                 h16* hidden, float* xres, cudaStream_t st, const SeqLayout& lay) {
+  const B2EModelDesc& d = e->desc;
+  const int M = B * S, H = d.hidden;
+  switch (d.arch) {
+    case B2E_ARCH_BERT:   // leading slots: word, position, token-type embeddings, embedding LayerNorm g/b
+      DISPATCH_H(H, (embed_layernorm_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                         ids, types, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2],
+                         (const float*)e->w[3], (const float*)e->w[4], hidden, M, S, d.eps, lay.t_real,
+                         lay.tok_src)));
+      break;
+    case B2E_ARCH_ESM2: {
+      const int mask_token = d.reserved - 1;  // reserved = mask_token_id + 1, 0 = token dropout off
+      esm_token_scale_kernel<<<(B + 7) / 8, 256, 0, st>>>(ids, mask, e->tok_scale, B, S, mask_token);
+      DISPATCH_H(H, (esm_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                         ids, mask, (const float*)e->w[0], e->tok_scale, xres, M, S, mask_token, lay.t_real,
+                         lay.tok_src)));
+      break;
+    }
+    case B2E_ARCH_MODERNBERT:
+      DISPATCH_H(H, (modernbert_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                         ids, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2], xres, hidden, M,
+                         d.eps, lay.t_real, lay.tok_src)));
+      break;
+    default:   // Mistral, Qwen3
+      DISPATCH_H(H, (mistral_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                         ids, (const float*)e->w[0], xres, M, lay.t_real, lay.tok_src)));
+  }
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
+}
+
 // Layers 0..L-1 up to (and including) the last FFN-down GEMM: leaves the pre-LayerNorm residual sum
 // of the final layer split as e->tmp (FFN-down output + bias) and e->hidden (the residual it still has
 // to be added to); every earlier LayerNorm output lives in e->hidden.
@@ -854,12 +889,7 @@ int run_bert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate;
   int rc;
-  // leading slots: word, position, token-type embeddings, embedding LayerNorm g/b
-  DISPATCH_H(H, (embed_layernorm_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     ids, types, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2],
-                     (const float*)e->w[3], (const float*)e->w[4], e->hidden, M, S, d.eps, lay.t_real,
-                     lay.tok_src)));
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_embed(e, ids, mask, types, B, S, e->hidden, nullptr, st, lay))) return rc;
 
   TrunkMaps tm;
   if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
@@ -902,13 +932,8 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const 
                   cudaStream_t st, const SeqLayout& lay) {
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
-  const int mask_token = d.reserved - 1;  // reserved = mask_token_id + 1, 0 = token dropout off
   int rc;
-  esm_token_scale_kernel<<<(B + 7) / 8, 256, 0, st>>>(ids, mask, e->tok_scale, B, S, mask_token);
-  DISPATCH_H(H, (esm_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     ids, mask, (const float*)e->w[0], e->tok_scale, e->xres, M, S, mask_token, lay.t_real,
-                     lay.tok_src)));
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_embed(e, ids, mask, nullptr, B, S, nullptr, e->xres, st, lay))) return rc;
   TrunkMaps tm;
   if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
 
@@ -956,9 +981,7 @@ int run_mistral_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, co
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   const int QC = e->qkv_cols(), CC = e->ctx_cols();
   int rc;
-  DISPATCH_H(H, (mistral_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     ids, (const float*)e->w[0], e->xres, M, lay.t_real, lay.tok_src)));
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_embed(e, ids, mask, nullptr, B, S, nullptr, e->xres, st, lay))) return rc;
   TrunkMaps tm;
   if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
 
@@ -1000,10 +1023,7 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
   int rc;
-  DISPATCH_H(H, (modernbert_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                     ids, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2], e->xres,
-                     e->hidden, M, d.eps, lay.t_real, lay.tok_src)));
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = launch_embed(e, ids, mask, nullptr, B, S, e->hidden, e->xres, st, lay))) return rc;
   TrunkMaps tm;
   if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
   for (int l = 0; l < L; ++l) {
@@ -1083,27 +1103,38 @@ int make_rope_tables(B2EEncoder* e) {
   return B2E_OK;
 }
 
-// The final norm of b2e_encode over the padded [B*S] rows, into float or the storage type.
+// One norm step over `rows` rows of width H into float or the storage type (n_dev: device row count, or null):
+// NORM_POST_LN LayerNorm(add + resid) of two 16-bit inputs (resid may be null), NORM_ADD_LN / NORM_ADD_RMS
+// xres += add (add may be null) in the fp32 residual stream, then LayerNorm / RMSNorm of xres (beta unused).
 template <typename OutT>
-int launch_final_norm(B2EEncoder* e, int M, OutT* out, cudaStream_t st) {
-  const B2EModelDesc& d = e->desc;
-  const float *g = e->final_norm(0), *b = e->final_norm(1);
-  switch (e->fam->norm) {
+int launch_norm(FinalNorm kind, int H, float* xres, const h16* add, const h16* resid, const float* g,
+                const float* b, OutT* out, int rows, float eps, cudaStream_t st, const int* n_dev = nullptr) {
+  switch (kind) {
     case NORM_POST_LN:
-      DISPATCH_H(d.hidden, (layernorm_kernel<HW, OutT><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                               e->tmp, e->hidden, g, b, out, M, d.eps)));
+      DISPATCH_H(H, (layernorm_kernel<HW, OutT><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
+                        add, resid, g, b, out, rows, eps, n_dev)));
       break;
-    case NORM_ADD_LN:   // emb_layer_norm_after / final_norm over (residual stream + last FFN output)
-      DISPATCH_H(d.hidden, (add_layernorm_kernel<HW, OutT><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                               e->xres, e->tmp, g, b, out, M, d.eps)));
+    case NORM_ADD_LN:
+      DISPATCH_H(H, (add_layernorm_kernel<HW, OutT><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
+                        xres, add, g, b, out, rows, eps, n_dev)));
       break;
-    case NORM_ADD_RMS:   // final RMSNorm over (residual stream + last down_proj output)
-      DISPATCH_H(d.hidden, (add_rmsnorm_kernel<HW, OutT><<<row_blocks(M), ROW_THREADS, 0, st>>>(
-                               e->xres, e->tmp, g, out, M, d.eps)));
+    case NORM_ADD_RMS:
+      DISPATCH_H(H, (add_rmsnorm_kernel<HW, OutT><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
+                        xres, add, g, out, rows, eps, n_dev)));
       break;
   }
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
+}
+
+// The final norm of b2e_encode over the padded [B*S] rows, into float or the storage type: BERT's last LayerNorm over
+// tmp + hidden, or emb_layer_norm_after / final_norm / the final RMSNorm over (residual stream + last FFN output).
+template <typename OutT>
+int launch_final_norm(B2EEncoder* e, int M, OutT* out, cudaStream_t st) {
+  const B2EModelDesc& d = e->desc;
+  const float *g = e->final_norm(0), *b = e->final_norm(1);
+  const h16* resid = e->fam->norm == NORM_POST_LN ? e->hidden.p : nullptr;
+  return launch_norm(e->fam->norm, d.hidden, e->xres, e->tmp, resid, g, b, out, M, d.eps, st);
 }
 
 }  // namespace
@@ -1798,6 +1829,23 @@ int b2e_debug_rotary(B2EEncoder* e, int layer, void* qkv, const int64_t* mask, i
   return B2E_OK;
 }
 
+// The handle's embedding step (launch_embed) into the caller's out16 / xres, in the token layout the encoder derives
+// from the mask, as b2e_debug_rotary.
+int b2e_debug_embed(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t* types, int B, int S,
+                    void* out16, float* xres, void* stream) {
+  int rc;
+  if ((rc = validate_batch(e, B, S))) return rc;
+  const int arch = e->desc.arch;
+  const bool wants16 = arch == B2E_ARCH_BERT || arch == B2E_ARCH_MODERNBERT, wants32 = arch != B2E_ARCH_BERT;
+  if (!ids || !mask || (wants16 && !out16) || (wants32 && !xres)) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = e->pack.ensure(B, (size_t)B * S))) return rc;
+  if (arch == B2E_ARCH_ESM2 && (rc = e->tok_scale.grow(B, e->ws_gen))) return rc;
+  SeqLayout lay;
+  if ((rc = pack_prepare(e->pack, mask, B, S, packing_enabled(), st, &lay))) return rc;
+  return launch_embed(e, ids, mask, types, B, S, (h16*)out16, xres, st, lay);
+}
+
 int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
                                int kv_heads, int head_dim, int window, int causal, void* stream) {
   if (!qkv || !mask || !ctx) return fail(B2E_ERR_INVALID, "null tensor pointer");
@@ -2122,17 +2170,30 @@ int b2e_layernorm(const void* in, const float* gamma, const float* beta, void* o
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  if (out_dtype == B2E_DTYPE_F32) {
-    DISPATCH_H(H, (layernorm_kernel<HW, float><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
-                       (const h16*)in, nullptr, gamma, beta, (float*)out, rows, eps)));
-  } else if (out_dtype == kStorageDtype) {
-    DISPATCH_H(H, (layernorm_kernel<HW, h16><<<row_blocks(rows), ROW_THREADS, 0, st>>>(
-                       (const h16*)in, nullptr, gamma, beta, (h16*)out, rows, eps)));
-  } else {
-    return fail(B2E_ERR_INVALID, "layernorm: out_dtype must be F32 or the storage type");
-  }
-  CUDA_TRY(cudaGetLastError());
-  return B2E_OK;
+  if (out_dtype == B2E_DTYPE_F32)
+    return launch_norm(NORM_POST_LN, H, nullptr, (const h16*)in, nullptr, gamma, beta, (float*)out, rows, eps, st);
+  if (out_dtype == kStorageDtype)
+    return launch_norm(NORM_POST_LN, H, nullptr, (const h16*)in, nullptr, gamma, beta, (h16*)out, rows, eps, st);
+  return fail(B2E_ERR_INVALID, "layernorm: out_dtype must be F32 or the storage type");
+}
+
+int b2e_debug_norm(int kind, int H, float* xres, const void* add, const void* resid, const float* gamma,
+                   const float* beta, void* out, int out_dtype, int rows, float eps, const int* t_real, void* stream) {
+  if (kind < NORM_POST_LN || kind > NORM_ADD_RMS) return fail(B2E_ERR_INVALID, "debug_norm: kind %d", kind);
+  const FinalNorm k = (FinalNorm)kind;
+  if (!gamma || !out || (k == NORM_POST_LN ? !add || !beta : !xres) || (k == NORM_ADD_LN && !beta))
+    return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (k != NORM_POST_LN && resid) return fail(B2E_ERR_INVALID, "debug_norm: the fp32-stream norms read no resid");
+  if (rows <= 0) return B2E_OK;
+  int rc;
+  if ((rc = check_h(H))) return rc;
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const h16 *a = (const h16*)add, *r = (const h16*)resid;
+  if (out_dtype == B2E_DTYPE_F32) return launch_norm(k, H, xres, a, r, gamma, beta, (float*)out, rows, eps, st, t_real);
+  if (out_dtype == kStorageDtype) return launch_norm(k, H, xres, a, r, gamma, beta, (h16*)out, rows, eps, st, t_real);
+  return fail(B2E_ERR_INVALID, "debug_norm: out_dtype must be F32 or the storage type");
 }
 
 }  // extern "C"

@@ -64,6 +64,19 @@ int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, 
  * the layer's q_norm / k_norm before rotating it.  Rows past the last attended token (packed layout) and the v
  * heads are not touched. */
 int b2e_debug_rotary(struct B2EEncoder* enc, int layer, void* qkv, const int64_t* mask, int B, int S, void* stream);
+/* the encoder's embedding step, in the token layout it derives from the mask (as b2e_debug_rotary), over B*S rows:
+ * BERT word + position + token-type embeddings and their LayerNorm into out16 (types may be NULL: type 0); ESM-2
+ * the token-dropout scale and the masked gather into xres; Mistral / Qwen3 the gather into xres; ModernBERT the
+ * gather and its LayerNorm into xres (fp32) and out16.  out16 is 16-bit storage [B*S, H], xres fp32 [B*S, H]; the
+ * one a family does not write may be NULL. */
+int b2e_debug_embed(struct B2EEncoder* enc, const int64_t* ids, const int64_t* mask, const int64_t* types, int B,
+                    int S, void* out16, float* xres, void* stream);
+/* one norm step of the trunks over `rows` rows of width H, with the caller's gamma / beta, into out (out_dtype: F32 or
+ * the storage type).  kind 0: LayerNorm(add + resid) over two 16-bit inputs (resid may be NULL); kind 1: xres += add
+ * in the fp32 residual stream, then LayerNorm of xres; kind 2: the same with RMSNorm (beta unused).  add may be NULL
+ * for kinds 1 and 2 (xres is only read).  t_real: device int whose value replaces rows, or NULL. */
+int b2e_debug_norm(int kind, int H, float* xres, const void* add, const void* resid, const float* gamma,
+                   const float* beta, void* out, int out_dtype, int rows, float eps, const int* t_real, void* stream);
 
 #ifdef __cplusplus
 }
