@@ -22,8 +22,11 @@ STORAGE_TORCH_DTYPE = {'f16': torch.float16, 'bf16': torch.bfloat16}
 # significand bits (tools/drift_report.py measures the drift per layer; tests/test_gpu_config_parity.py holds every
 # family to the tolerance at configuration depth).  bench.py's extra.storage_ab times the same GEMM in both builds.
 # Qwen3 follows Mistral: Qwen3-Embedding-4B / 8B are 36 layers deep.
+# ESM C runs bfloat16, as the reference does: at the esmc-600m shape (36 layers, S = 2048) its pooled rows stay within
+# 1 - cos 5.1e-5 of the fp32 restatement (half: 9.6e-7), a twentieth of the tolerance (README, tools/drift_report.py).
 # B2E_STORAGE=f16|bf16 overrides for every family.
-_STORAGE_BY_ARCH = {'bert': 'bf16', 'esm': 'bf16', 'modernbert': 'bf16', 'mistral': 'f16', 'qwen3': 'f16'}
+_STORAGE_BY_ARCH = {'bert': 'bf16', 'esm': 'bf16', 'modernbert': 'bf16', 'mistral': 'f16', 'qwen3': 'f16',
+                   'esmc': 'bf16'}
 
 
 def storage_for_arch(arch: str) -> str:
@@ -44,7 +47,7 @@ def storage_of(dtype: torch.dtype) -> str:
             return name
     raise NativeError(f'no libb2e build stores {dtype}: expected float16 or bfloat16 operands')
 
-ARCH_BERT, ARCH_ESM2, ARCH_MISTRAL, ARCH_MODERNBERT, ARCH_QWEN3 = 0, 1, 2, 3, 4
+ARCH_BERT, ARCH_ESM2, ARCH_MISTRAL, ARCH_MODERNBERT, ARCH_QWEN3, ARCH_ESMC = 0, 1, 2, 3, 4, 5
 DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2
 POOL_MEAN_REF, POOL_MEAN_PER_ROW, POOL_LAST_TOKEN = 0, 1, 2
 EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESID, EPI_SWIGLU, EPI_GEGLU = 0, 1, 2, 3, 4
@@ -78,6 +81,7 @@ EXPORTS = (
     'b2e_attention_d64_window',
     'b2e_attention_causal_d128',
     'b2e_qk_norm_rope',
+    'b2e_qk_layernorm_rope',
     'b2e_topk_ip',
     'b2e_topk_ip_tc',
     'b2e_max_row_norm',
@@ -188,6 +192,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_attention_causal_d128.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
     lib.b2e_qk_norm_rope.restype = i32
     lib.b2e_qk_norm_rope.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, C.c_float, vp, vp, vp]
+    lib.b2e_qk_layernorm_rope.restype = i32
+    lib.b2e_qk_layernorm_rope.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, C.c_float, vp, vp, vp]
     lib.b2e_topk_ip.restype = i32
     lib.b2e_topk_ip.argtypes = [vp, i32, vp, i32, i64, i32, i32, vp, vp, vp]
     lib.b2e_topk_ip_tc.restype = i32
@@ -512,6 +518,31 @@ def qk_norm_rope_(qkv: torch.Tensor, q_gamma: torch.Tensor, k_gamma: torch.Tenso
         check(lib.b2e_qk_norm_rope(qkv.data_ptr(), q_gamma.data_ptr(), k_gamma.data_ptr(), cos.data_ptr(),
                                    sin.data_ptr(), qkv.shape[0], cos.shape[0], heads, kv_heads, eps, _ptr(t_real),
                                    _ptr(tok_src), stream_ptr(qkv.device)), lib)
+    return qkv
+
+
+def qk_layernorm_rope_(qkv: torch.Tensor, q_gamma: torch.Tensor, k_gamma: torch.Tensor, cos: torch.Tensor,
+                       sin: torch.Tensor, eps: float, t_real: torch.Tensor | None = None,
+                       tok_src: torch.Tensor | None = None) -> torch.Tensor:
+    """ESM C's q/k step in place on qkv [T, 3H] (q | k | v, H = 960 or 1152): a LayerNorm without bias over the whole
+    q row (gain q_gamma, fp32 [H]) and the whole k row (k_gamma), then rotary per 64-wide head with cos / sin [S, 32]
+    fp32 at position tok_src[t] % S (or t % S).  ``t_real``: int32 device tensor whose first element replaces T as
+    the row count."""
+    lib = load(storage_of(qkv.dtype))
+    for t, what in ((qkv, 'qkv'), (q_gamma, 'q_gamma'), (k_gamma, 'k_gamma'), (cos, 'cos'), (sin, 'sin')):
+        _cuda_contig(t, what)
+    for t, what in ((t_real, 't_real'), (tok_src, 'tok_src')):
+        if t is not None and (_cuda_contig(t, what).dtype != torch.int32):
+            raise NativeError(f'{what} must be int32')
+    if any(t.dtype != torch.float32 for t in (q_gamma, k_gamma, cos, sin)):
+        raise NativeError('gains and rotary tables must be float32')
+    h = qkv.shape[1] // 3
+    if qkv.shape[1] != 3 * h or cos.shape[1] != 32 or q_gamma.numel() != h or k_gamma.numel() != h:
+        raise NativeError('qk_layernorm_rope_: expected qkv [T, 3H], tables [S, 32], gains [H]')
+    with torch.cuda.device(qkv.device):
+        check(lib.b2e_qk_layernorm_rope(qkv.data_ptr(), q_gamma.data_ptr(), k_gamma.data_ptr(), cos.data_ptr(),
+                                        sin.data_ptr(), qkv.shape[0], cos.shape[0], h, eps, _ptr(t_real),
+                                        _ptr(tok_src), stream_ptr(qkv.device)), lib)
     return qkv
 
 

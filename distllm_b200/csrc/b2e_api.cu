@@ -189,9 +189,11 @@ int ensure_smem_attr(Kern kern, int bytes) {
 }
 
 // ---------------------------------------------------------------- launches
-int check_gemm_shape(int M, int N, int K) {
+// wide: the GEMM runs 16-bit weights with a non-gated epilogue, so the 192-wide tile kernel exists for it (gemm_bn) and
+// also covers an N that is a multiple of 192 but not of 128 (ESMC-300m's N = 960 and 2880)
+int check_gemm_shape(int M, int N, int K, bool wide = false) {
   if (M <= 0 || N <= 0 || K <= 0) return fail(B2E_ERR_INVALID, "gemm: empty shape %dx%dx%d", M, N, K);
-  if (N % 128 != 0) return fail(B2E_ERR_INVALID, "gemm: N=%d must be a multiple of 128", N);
+  if (N % 128 != 0 && !(wide && N % 192 == 0)) return fail(B2E_ERR_INVALID, "gemm: N=%d must be a multiple of 128", N);
   if (K % 64 != 0) return fail(B2E_ERR_INVALID, "gemm: K=%d must be a multiple of 64", K);
   return B2E_OK;
 }
@@ -211,12 +213,13 @@ inline int gemm_bn_override() {
 }
 
 // The tile width of the GEMM whose W has N rows (gemm.cuh): 192 wherever that kernel exists (16-bit weights, not a
-// gated epilogue) and divides N, else 128.
+// gated epilogue) and divides N, else 128.  The override applies only where its width divides N: an N that is a
+// multiple of 192 but not of 128 has no 128-wide kernel.
 int gemm_bn(int N, int epi, bool nf4) {
   const bool wide_ok = !nf4 && epi != B2E_EPI_SWIGLU && epi != B2E_EPI_GEGLU && N % 192 == 0;
   if (!wide_ok) return 128;
   const int forced = gemm_bn_override();
-  return forced ? forced : 192;
+  return forced && N % forced == 0 ? forced : 192;
 }
 
 // The W operand of a GEMM: a 16-bit [N,K] map (box 64 x bn), or with absmax set the NF4 code map
@@ -547,7 +550,7 @@ int launch_attention_bidir(const CUtensorMap& tqkv, const AttnScratch& sc, void*
 }
 
 // Row kernels are instantiated per hidden width HW (rowops.cuh: row_passes / row_lane_on); check_h accepts exactly
-// these widths.
+// these widths but ESMC's 960 and 1152, which only ESMC and the standalone row entry points accept (check_row_h).
 #define DISPATCH_H(H, CALL)                                         \
   switch (H) {                                                      \
     case 256: { constexpr int HW = 256; CALL; break; }              \
@@ -555,7 +558,9 @@ int launch_attention_bidir(const CUtensorMap& tqkv, const AttnScratch& sc, void*
     case 512: { constexpr int HW = 512; CALL; break; }              \
     case 640: { constexpr int HW = 640; CALL; break; }              \
     case 768: { constexpr int HW = 768; CALL; break; }              \
+    case 960: { constexpr int HW = 960; CALL; break; }              \
     case 1024: { constexpr int HW = 1024; CALL; break; }            \
+    case 1152: { constexpr int HW = 1152; CALL; break; }            \
     case 1280: { constexpr int HW = 1280; CALL; break; }            \
     case 2048: { constexpr int HW = 2048; CALL; break; }            \
     case 2560: { constexpr int HW = 2560; CALL; break; }            \
@@ -575,6 +580,12 @@ int check_h(int H) {
   }
   return fail(B2E_ERR_UNSUPPORTED, "hidden size %d not supported (built: 256 x {1,2,3,4,5,8,10,16}, 384, 640)", H);
 }
+
+// ESM C's widths (esmc-300m, esmc-600m): a 192-column and a 128-column last pass
+inline bool esmc_width(int H) { return H == 960 || H == 1152; }
+
+// The widths of the standalone row entry points (pool_mean, layernorm, debug_norm): every width DISPATCH_H builds
+int check_row_h(int H) { return esmc_width(H) ? B2E_OK : check_h(H); }
 
 // Pool-weight scratch shared by the fused and the standalone poolers.
 struct PoolScratch : DeviceScratch {
@@ -816,12 +827,40 @@ int trunk_prologue(B2EEncoder* e, const int64_t* mask, int B, int S, cudaStream_
   return make_tmap_h16(&tm->qkv, e->qkv, M, e->qkv_cols(), AT_KC, d.head_dim);
 }
 
+// ESMC's q / k LayerNorm fused with the rotation (qk_layernorm_rope_kernel), one warp per q or k row of qkv [T, 3H];
+// instantiated for the ESMC widths only.
+int launch_qk_layernorm_rope(int H, h16* qkv, const float* q_gamma, const float* k_gamma, const float* cos_t,
+                             const float* sin_t, int T, int S, float eps, const int* n_dev, const int* tok_src,
+                             cudaStream_t st) {
+  const unsigned grid = (unsigned)row_blocks(2 * T);
+  switch (H) {
+    case 960:
+      qk_layernorm_rope_kernel<960><<<grid, ROW_THREADS, 0, st>>>(qkv, q_gamma, k_gamma, cos_t, sin_t, T, S, eps,
+                                                                  n_dev, tok_src);
+      break;
+    case 1152:
+      qk_layernorm_rope_kernel<1152><<<grid, ROW_THREADS, 0, st>>>(qkv, q_gamma, k_gamma, cos_t, sin_t, T, S, eps,
+                                                                   n_dev, tok_src);
+      break;
+    default:
+      return fail(B2E_ERR_INVALID, "qk_layernorm_rope: hidden size %d not built (built: 960, 1152)", H);
+  }
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
+}
+
 // The rotary step of layer l, in place on qkv [M, qkv_cols()] in the token layout `lay` (rows from lay.t_real on are
 // not touched): ESM-2 rope_halves<16> (head_dim 32) or <32> over its q and k heads, ModernBERT rope_halves<32> with the
 // full-attention (l % global_every == 0) or the sliding-attention table, Mistral rope_halves<64>, Qwen3 the per-head
-// q / k RMSNorm fused with the rotation.  The trunks and b2e_debug_rotary launch it.
+// q / k RMSNorm fused with the rotation, ESMC the full-width q / k LayerNorm fused with it.  The trunks and
+// b2e_debug_rotary launch it.
 void launch_rotary(B2EEncoder* e, int l, h16* qkv, int M, int S, cudaStream_t st, const SeqLayout& lay) {
   const B2EModelDesc& d = e->desc;
+  if (d.arch == B2E_ARCH_ESMC) {   // (b2e_check_model accepted the width)
+    launch_qk_layernorm_rope(d.hidden, qkv, (const float*)e->slot(l, 3), (const float*)e->slot(l, 4), e->rope_cos,
+                             e->rope_sin, M, S, d.eps, lay.t_real, lay.tok_src, st);
+    return;
+  }
   if (is_decoder(d.arch)) {
     const int n_rot = d.heads + d.kv_heads;   // q heads and k heads are adjacent columns of qkv
     const unsigned grid = (unsigned)(((long long)M * n_rot * 8 + 255) / 256);
@@ -847,7 +886,7 @@ void launch_rotary(B2EEncoder* e, int l, h16* qkv, int M, int S, cudaStream_t st
 }
 
 // The embedding step of a family over M = B*S rows in the token layout `lay`: BERT embed_layernorm into hidden, ESM-2
-// the token-dropout scales (into e->tok_scale) and esm_embed into xres, Mistral / Qwen3 the gather into xres,
+// the token-dropout scales (into e->tok_scale) and esm_embed into xres, Mistral / Qwen3 / ESMC the gather into xres,
 // ModernBERT the gather into xres and its LayerNorm into hidden.  The trunks and b2e_debug_embed launch it.
 int launch_embed(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t* types, int B, int S,
                  h16* hidden, float* xres, cudaStream_t st, const SeqLayout& lay) {
@@ -873,7 +912,7 @@ int launch_embed(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const i
                          ids, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2], xres, hidden, M,
                          d.eps, lay.t_real, lay.tok_src)));
       break;
-    default:   // Mistral, Qwen3
+    default:   // Mistral, Qwen3, ESMC
       DISPATCH_H(H, (mistral_embed_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          ids, (const float*)e->w[0], xres, M, lay.t_real, lay.tok_src)));
   }
@@ -958,6 +997,51 @@ int run_esm_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const 
       return rc;
     if ((rc = launch_gemm(tm.ffn, e->tm_w2[l], e->tmp, (const float*)e->slot(l, 11), nullptr, M, H, I,
                           B2E_EPI_BIAS, st, lay.t_real)))
+      return rc;
+    if (l + 1 < L) {
+      DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                         e->xres, e->tmp, (const float*)e->slot(l + 1, 0), (const float*)e->slot(l + 1, 1),
+                         e->hidden, M, d.eps, lay.t_real)));
+    }
+  }
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
+}
+
+// ESM C (esm/models/esmc.py, esm/layers/blocks.py and attention.py of the esm package): pre-LayerNorm blocks without
+// Linear biases, a LayerNorm over the whole q row and the whole k row before the rotary embedding (launch_rotary),
+// bidirectional head_dim-64 attention with the key-padding bias, SwiGLU.  The checkpoint's residual scale 1/sqrt(L/36)
+// is folded into Wo and W2 when the weights are built (embed/encoders/weights.py: esmc_weight_list), so the block is
+// the ESM-2 trunk's sequence of steps.  Leaves xres (before the last FFN output is added) and e->tmp (that output): the
+// caller applies transformer.norm to xres + tmp.
+int run_esmc_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const int64_t*, int B, int S,
+                   cudaStream_t st, const SeqLayout& lay) {
+  const B2EModelDesc& d = e->desc;
+  const int M = B * S, H = d.hidden, I = d.intermediate, L = d.num_layers;
+  int rc;
+  if ((rc = launch_embed(e, ids, mask, nullptr, B, S, nullptr, e->xres, st, lay))) return rc;
+  TrunkMaps tm;
+  if ((rc = trunk_prologue(e, mask, B, S, st, &tm))) return rc;
+
+  DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                     e->xres, nullptr, (const float*)e->slot(0, 0), (const float*)e->slot(0, 1), e->hidden,
+                     M, d.eps, lay.t_real)));
+  for (int l = 0; l < L; ++l) {
+    if ((rc = launch_gemm(tm.hidden, e->tm_wqkv[l], e->qkv, nullptr, nullptr, M, 3 * H, H, B2E_EPI_BIAS, st, lay.t_real)))
+      return rc;
+    launch_rotary(e, l, e->qkv, M, S, st, lay);
+    if ((rc = launch_attention_bidir(tm.qkv, e->attn, e->ctx, B, S, d.heads, d.head_dim, st, lay)))
+      return rc;
+    if ((rc = launch_gemm(tm.ctx, e->tm_wo[l], e->tmp, nullptr, nullptr, M, H, H, B2E_EPI_BIAS, st, lay.t_real)))
+      return rc;
+    DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
+                       e->xres, e->tmp, (const float*)e->slot(l, 6), (const float*)e->slot(l, 7), e->hidden,
+                       M, d.eps, lay.t_real)));
+    // gate and up in one GEMM (interleaved rows), silu(gate) * up in its epilogue: [M, I]
+    if ((rc = launch_gemm(tm.hidden, e->tm_w1[l], e->ffn, nullptr, nullptr, M, 2 * I, H, B2E_EPI_SWIGLU, st,
+                          lay.t_real)))
+      return rc;
+    if ((rc = launch_gemm(tm.ffn, e->tm_w2[l], e->tmp, nullptr, nullptr, M, H, I, B2E_EPI_BIAS, st, lay.t_real)))
       return rc;
     if (l + 1 < L) {
       DISPATCH_H(H, (add_layernorm_kernel<HW, h16><<<row_blocks(M), ROW_THREADS, 0, st>>>(
@@ -1064,6 +1148,8 @@ int run_modernbert_trunk(B2EEncoder* e, const int64_t* ids, const int64_t* mask,
 //   ModernBERT  0 tok_embeddings, 1/2 embeddings.norm g/b, 3/4 final_norm g/b; per layer (5 + 8 l): attn_norm g/b,
 //               Wqkv, Wo, mlp_norm g/b, Wi (input/gate interleaved), mlp.Wo
 //   Qwen3       Mistral's, with q_norm, k_norm (fp32 [128]) after the six of each layer (2 + 8 l)
+//   ESMC        0 embed, 1/2 final norm g/b (b: zeros); per layer (3 + 10 l): ln_qkv g/b, Wqkv, q_ln, k_ln (fp32 [H]),
+//               Wo, ffn LayerNorm g/b, W1 (gate/up interleaved), W2
 // Indexed by B2E_ARCH_*.
 constexpr Family kFamilies[] = {
     {5, 12, 0, 2, 6, 8, false, B2E_EPI_BIAS_GELU, NORM_POST_LN, 10, 11, run_bert_trunk},        // B2E_ARCH_BERT
@@ -1071,6 +1157,7 @@ constexpr Family kFamilies[] = {
     {2, 6, 1, 2, 4, 5, true, B2E_EPI_SWIGLU, NORM_ADD_RMS, 1, -1, run_mistral_trunk},          // B2E_ARCH_MISTRAL
     {5, 8, 2, 3, 6, 7, true, B2E_EPI_GEGLU, NORM_ADD_LN, 3, 4, run_modernbert_trunk},          // B2E_ARCH_MODERNBERT
     {2, 8, 1, 2, 4, 5, true, B2E_EPI_SWIGLU, NORM_ADD_RMS, 1, -1, run_mistral_trunk},          // B2E_ARCH_QWEN3
+    {3, 10, 2, 5, 8, 9, true, B2E_EPI_SWIGLU, NORM_ADD_LN, 1, 2, run_esmc_trunk},              // B2E_ARCH_ESMC
 };
 
 const Family* family(int arch) {
@@ -1080,7 +1167,8 @@ const Family* family(int arch) {
 // Rotary cos / sin tables [max_pos, cols] of the families that rotate q and k, built once.  Each table's kernel and
 // arguments decide results bit for bit: ESM-2 at head_dim 64 keeps rope_table_kernel, ESM-2 at head_dim 32 builds
 // angle(p, i) = p * 10000^(-2i/32) over 16 columns, ModernBERT one table per layer type (rope_theta for the
-// full-attention layers, rope_theta_local for the sliding ones), Mistral / Qwen3 64 columns of rope_theta.
+// full-attention layers, rope_theta_local for the sliding ones), Mistral / Qwen3 64 columns of rope_theta, ESMC 32
+// columns of rope_theta.
 int make_rope_tables(B2EEncoder* e) {
   const B2EModelDesc& d = e->desc;
   if (d.arch == B2E_ARCH_BERT) return B2E_OK;
@@ -1229,6 +1317,20 @@ int b2e_check_model(const B2EModelDesc* desc) {
     if ((rc = check_gemm_shape(128, 2 * I, H))) return rc;
     return check_gemm_shape(128, H, I);
   }
+  if (desc->arch == B2E_ARCH_ESMC) {
+    const int H = desc->hidden, I = desc->intermediate;
+    if (desc->head_dim != 64 || desc->heads * 64 != H)
+      return fail(B2E_ERR_UNSUPPORTED, "ESMC: need head_dim 64 and heads*64 == hidden (got %d heads x %d, H=%d)",
+                  desc->heads, desc->head_dim, H);
+    if (!esmc_width(H)) return fail(B2E_ERR_UNSUPPORTED, "ESMC: hidden size %d not built (built: 960, 1152)", H);
+    if (I % 128 != 0)
+      return fail(B2E_ERR_UNSUPPORTED, "ESMC: intermediate size %d must be a multiple of 128", I);
+    // Wqkv, Wo and W2 run the 192-wide tile where 128 does not divide N; the gated W1 runs 128-wide tiles
+    if ((rc = check_gemm_shape(128, 3 * H, H, true))) return rc;
+    if ((rc = check_gemm_shape(128, H, H, true))) return rc;
+    if ((rc = check_gemm_shape(128, 2 * I, H))) return rc;
+    return check_gemm_shape(128, H, I, true);
+  }
   if (desc->arch != B2E_ARCH_BERT && desc->arch != B2E_ARCH_ESM2 && desc->arch != B2E_ARCH_MODERNBERT)
     return fail(B2E_ERR_UNSUPPORTED, "arch %d: unknown architecture", desc->arch);
   if (desc->arch == B2E_ARCH_MODERNBERT) {
@@ -1264,6 +1366,9 @@ int create_encoder(const B2EModelDesc* desc, const void* const* weights, int n_w
   *out = nullptr;
   int rc;
   if ((rc = b2e_check_model(desc))) return rc;
+  // ESMC-300m's N = 960 / 2880 GEMMs exist as 192-wide 16-bit kernels only; no ESMC configuration is quantised
+  if (absmax && desc->arch == B2E_ARCH_ESMC)
+    return fail(B2E_ERR_UNSUPPORTED, "ESMC: NF4 weights are not built (built: 16-bit weights)");
   if (n_weights != b2e_num_weights(desc))
     return fail(B2E_ERR_INVALID, "expected %d weight pointers, got %d", b2e_num_weights(desc), n_weights);
   for (int i = 0; i < n_weights; ++i)
@@ -1552,7 +1657,7 @@ int b2e_pool_mean(const void* hidden, int dtype, int64_t* mask, int B, int S, in
   if (pool_kind != B2E_POOL_MEAN_REF && pool_kind != B2E_POOL_MEAN_PER_ROW)
     return fail(B2E_ERR_INVALID, "pool_mean: pool_kind %d", pool_kind);
   int rc;
-  if ((rc = check_h(H))) return rc;
+  if ((rc = check_row_h(H))) return rc;
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1671,7 +1776,7 @@ int gemm_entry(const void* A, const void* W, const float* absmax, const float* b
   if (epi != B2E_EPI_BIAS_RESID && resid) return fail(B2E_ERR_INVALID, "gemm: epilogue %d reads no resid", epi);
   if (epi_is_glu(epi) && bias) return fail(B2E_ERR_INVALID, "gemm: the gated epilogues add no bias");
   int rc;
-  if ((rc = check_gemm_shape(M, N, K))) return rc;
+  if ((rc = check_gemm_shape(M, N, K, !absmax && !epi_is_glu(epi)))) return rc;
   if (epi_is_glu(epi) && N % 256 != 0)
     return fail(B2E_ERR_INVALID, "gemm: the gated epilogues need N %% 256 == 0 (got %d)", N);
   DeviceInfo info;
@@ -1792,6 +1897,20 @@ int b2e_qk_norm_rope(void* qkv, const float* q_gamma, const float* k_gamma, cons
       eps, t_real, tok_src);
   CUDA_TRY(cudaGetLastError());
   return B2E_OK;
+}
+
+int b2e_qk_layernorm_rope(void* qkv, const float* q_gamma, const float* k_gamma, const float* cos_t,
+                          const float* sin_t, int T, int S, int H, float eps, const int* t_real, const int* tok_src,
+                          void* stream) {
+  if (!qkv || !q_gamma || !k_gamma || !cos_t || !sin_t) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (T <= 0 || S <= 0) return fail(B2E_ERR_INVALID, "qk_layernorm_rope: bad problem T=%d S=%d", T, S);
+  if (!esmc_width(H)) return fail(B2E_ERR_INVALID, "qk_layernorm_rope: hidden size %d not built (built: 960, 1152)", H);
+  if (T > 0x3fffffff) return fail(B2E_ERR_INVALID, "qk_layernorm_rope: %d rows", T);
+  int rc;
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  return launch_qk_layernorm_rope(H, static_cast<h16*>(qkv), q_gamma, k_gamma, cos_t, sin_t, T, S, eps, t_real,
+                                  tok_src, (cudaStream_t)stream);
 }
 
 int b2e_attention_causal_d128(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,
@@ -2166,7 +2285,7 @@ int b2e_layernorm(const void* in, const float* gamma, const float* beta, void* o
   if (!in || !gamma || !beta || !out) return fail(B2E_ERR_INVALID, "null tensor pointer");
   if (rows <= 0) return B2E_OK;
   int rc;
-  if ((rc = check_h(H))) return rc;
+  if ((rc = check_row_h(H))) return rc;
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -2186,7 +2305,7 @@ int b2e_debug_norm(int kind, int H, float* xres, const void* add, const void* re
   if (k != NORM_POST_LN && resid) return fail(B2E_ERR_INVALID, "debug_norm: the fp32-stream norms read no resid");
   if (rows <= 0) return B2E_OK;
   int rc;
-  if ((rc = check_h(H))) return rc;
+  if ((rc = check_row_h(H))) return rc;
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
   cudaStream_t st = (cudaStream_t)stream;

@@ -257,4 +257,48 @@ qk_rmsnorm_rope_kernel(h16* __restrict__ qkv, const float* __restrict__ q_gamma,
   store8(p + HALF, o2);
 }
 
+// ESM C (esm/layers/attention.py, esm/layers/rotary.py of the esm package): the whole H-wide q row and the whole k row
+// of qkv [T, 3H] each go through a LayerNorm without bias (q_ln / k_ln, statistics over H in fp32), and then every
+// 64-wide head of the result is rotated in the halves convention at position tok_src[t] % S (or t % S), in place:
+//   y = gamma * ((x - mean) * rstd);  out[i] = y[i] cos_i - y[i+32] sin_i,  out[i+32] = y[i+32] cos_i + y[i] sin_i
+// One warp per (token, q or k) row in the row layout of rowops.cuh (warp_layernorm): lane owns 8 consecutive columns
+// of each 256-column pass, so a head is 8 lanes of one pass and the partner of a lane's columns is lane ^ 4 (the same
+// 8 frequencies (lane & 3) * 8 .. +8 of the other half).  Heads never straddle a pass, and the off lanes of a partial
+// pass (row_lane_on) hold whole heads, so an on lane never partners an off lane.  One rounding to 16 bits, at the
+// store; V and rows from T on (T = *n_dev when given) are not touched.
+template <int H>
+__global__ void __launch_bounds__(ROW_THREADS)
+qk_layernorm_rope_kernel(h16* __restrict__ qkv, const float* __restrict__ q_gamma, const float* __restrict__ k_gamma,
+                         const float* __restrict__ cos_t, const float* __restrict__ sin_t, int T, int S, float eps,
+                         const int* __restrict__ n_dev = nullptr, const int* __restrict__ tok_src = nullptr) {
+  constexpr int NV = row_passes(H), HALF = 32;
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5);   // 2 t + (0: q, 1: k)
+  if (n_dev != nullptr) T = __ldg(n_dev);
+  const int t = r >> 1;
+  if (t >= T) return;   // warp-uniform
+  h16* row = qkv + static_cast<size_t>(t) * (3 * H) + (r & 1) * H;
+  float x[NV][8];
+#pragma unroll
+  for (int v = 0; v < NV; ++v)
+    if (row_lane_on<H>(v, lane)) load8(row + v * 256 + lane * 8, x[v]);
+    else zero8(x[v]);
+  warp_layernorm<H, false>(x, (r & 1) ? k_gamma : q_gamma, nullptr, lane, eps);
+  const int pos = (tok_src != nullptr ? __ldg(tok_src + t) : t) % S;
+  float c[8], sn[8];
+  load8(cos_t + static_cast<size_t>(pos) * HALF + (lane & 3) * 8, c);
+  load8(sin_t + static_cast<size_t>(pos) * HALF + (lane & 3) * 8, sn);
+  const bool upper = (lane & 4) != 0;   // columns i + 32 of the head
+#pragma unroll
+  for (int v = 0; v < NV; ++v) {
+    float o[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float p = __shfl_xor_sync(0xffffffffu, x[v][e], 4);
+      o[e] = upper ? x[v][e] * c[e] + p * sn[e] : x[v][e] * c[e] - p * sn[e];
+    }
+    if (row_lane_on<H>(v, lane)) store8(row + v * 256 + lane * 8, o);
+  }
+}
+
 }  // namespace b2e

@@ -14,14 +14,15 @@ constexpr int ROW_WARPS = 8;
 constexpr int ROW_THREADS = ROW_WARPS * 32;
 
 // A row of H columns is held as row_passes(H) passes of 256 columns, lane owning columns v*256 + lane*8 .. +8 of
-// pass v.  The row kernels are instantiated per H (DISPATCH_H): 256 x {1,2,3,4,5,8,10,16}, 384 and 640.  A width with
-// a 128-column remainder ends on a half pass: there lanes 16-31 are off (row_lane_on), hold zeros, load and store
-// nothing and add nothing to the row statistics, which still divide by H.  For H % 256 == 0 the predicate is the
-// constant true and the kernels are the same code as with whole passes only.
+// pass v.  The row kernels are instantiated per H (DISPATCH_H): 256 x {1,2,3,4,5,8,10,16}, 384, 640, 960 and 1152.  A
+// width with a remainder ends on a partial pass of (H % 256) / 8 lanes: a 128-column half pass (384, 640, 1152: lanes
+// 16-31 off) or a 192-column pass (960: lanes 24-31 off).  Off lanes (row_lane_on) hold zeros, load and store nothing
+// and add nothing to the row statistics, which still divide by H.  For H % 256 == 0 the predicate is the constant true
+// and the kernels are the same code as with whole passes only.
 __host__ __device__ constexpr int row_passes(int H) { return (H + 255) / 256; }
 template <int H>
 __device__ __forceinline__ bool row_lane_on(int v, int lane) {
-  return H % 256 == 0 || v < H / 256 || lane < 16;
+  return H % 256 == 0 || v < H / 256 || lane < (H % 256) / 8;
 }
 
 // ---- 8-element vector load/store helpers (lane owns columns v*256 + lane*8 .. +8)
@@ -76,8 +77,8 @@ __device__ __forceinline__ void zero8(float (&v)[8]) {   // the values of an off
 }
 
 // LayerNorm of one row held as NV x 8 values per lane (biased variance, like torch.layer_norm); the values of off
-// lanes (row_lane_on) are zeros.
-template <int H>
+// lanes (row_lane_on) are zeros.  BIAS == false: no bias (ESMC's q_ln / k_ln), beta is not read.
+template <int H, bool BIAS = true>
 __device__ __forceinline__ void warp_layernorm(float (&x)[row_passes(H)][8], const float* __restrict__ gamma,
                                                const float* __restrict__ beta, int lane, float eps) {
   constexpr int NV = row_passes(H);
@@ -104,11 +105,17 @@ __device__ __forceinline__ void warp_layernorm(float (&x)[row_passes(H)][8], con
 #pragma unroll
   for (int v = 0; v < NV; ++v) {
     if (!row_lane_on<H>(v, lane)) continue;
-    float g[8], b[8];
+    float g[8];
     load8(gamma + v * 256 + lane * 8, g);
-    load8(beta + v * 256 + lane * 8, b);
+    if constexpr (BIAS) {
+      float b[8];
+      load8(beta + v * 256 + lane * 8, b);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) x[v][e] = fmaf((x[v][e] - mean) * rstd, g[e], b[e]);
+      for (int e = 0; e < 8; ++e) x[v][e] = fmaf((x[v][e] - mean) * rstd, g[e], b[e]);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) x[v][e] = ((x[v][e] - mean) * rstd) * g[e];
+    }
   }
 }
 

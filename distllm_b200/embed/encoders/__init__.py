@@ -1,5 +1,5 @@
-"""Encoder family: ``auto`` (BERT-family checkpoints) and ``esm2``, both on the native kernels.
-``esmc`` (needs the ``esm`` package) is not provided."""
+"""Encoder family: ``auto`` (BERT-family checkpoints), ``esm2`` and ``esmc`` (ESM C), all on the native kernels.
+``esmc`` reads the checkpoint's state dict directly: the ``esm`` package is not needed."""
 
 from __future__ import annotations
 
@@ -12,13 +12,16 @@ from distllm_b200.embed.encoders.auto import AutoEncoderConfig
 from distllm_b200.embed.encoders.base import Encoder
 from distllm_b200.embed.encoders.esm2 import Esm2Encoder
 from distllm_b200.embed.encoders.esm2 import Esm2EncoderConfig
+from distllm_b200.embed.encoders.esmc import EsmCambrianEncoder
+from distllm_b200.embed.encoders.esmc import EsmCambrianEncoderConfig
 from distllm_b200.registry import registry
 from distllm_b200.utils import BaseConfig
 
-EncoderConfigs = Union[Esm2EncoderConfig, AutoEncoderConfig]
+EncoderConfigs = Union[Esm2EncoderConfig, EsmCambrianEncoderConfig, AutoEncoderConfig]
 
 STRATEGIES: dict[str, tuple[type[BaseConfig], type[Encoder]]] = {
     'esm2': (Esm2EncoderConfig, Esm2Encoder),
+    'esmc': (EsmCambrianEncoderConfig, EsmCambrianEncoder),
     'auto': (AutoEncoderConfig, AutoEncoder),
 }
 

@@ -32,8 +32,8 @@ class NativeBertEncoder:
 
         ``lora`` (NF4 only; ``adapters.Adapter.lora``): LoRA modules kept unmerged, added by the NF4 GEMMs as extra
         k-blocks (``b2e_encoder_create_nf4_lora``, ``weights.lora_slot_factors``)."""
-        if nf4 and self._ARCH == 'esm':
-            raise NotImplementedError('ESM-2 has no quantised configuration')
+        if nf4 and self._ARCH in ('esm', 'esmc'):
+            raise NotImplementedError('ESM-2 and ESM C have no quantised configuration')
         if lora and not nf4:
             raise ValueError('unmerged LoRA needs NF4 storage; merge the adapter into 16-bit weights instead')
         self.storage = storage or _native.storage_for_arch(self._ARCH)
@@ -218,3 +218,13 @@ class NativeModernBertEncoder(NativeBertEncoder):
     _DESC = staticmethod(W.modernbert_desc)
     _WEIGHTS = staticmethod(W.modernbert_weight_list)
     _ARCH = 'modernbert'
+
+
+class NativeEsmcEncoder(NativeBertEncoder):
+    """ESM C (esmc-300m, esmc-600m): pre-LayerNorm blocks, a LayerNorm over the whole q and k rows fused with the
+    rotary embedding, bidirectional head_dim-64 attention, SwiGLU.  ``hf_config`` is a ``weights.EsmcConfig`` read
+    from the checkpoint's shapes (``weights.esmc_config``); ``token_type_ids`` unused."""
+
+    _DESC = staticmethod(W.esmc_desc)
+    _WEIGHTS = staticmethod(W.esmc_weight_list)
+    _ARCH = 'esmc'

@@ -753,3 +753,170 @@ def lora_slot_factors(arch: str, hf_config, lora: Mapping[str, tuple[torch.Tenso
     if missing:
         raise ValueError(f'LoRA modules outside the GEMM slots of {arch}: {missing[:8]}')
     return out
+
+
+# ------------------------------------------------------------------------------ ESM C
+# ESM C (``B2E_ARCH_ESMC``), 3 + 10*L device tensors, from the esm package's state dict (esm/models/esmc.py,
+# esm/layers/blocks.py, attention.py; ``esmc_{300m,600m}_2024_12_v0.pth``), no Linear biases:
+#
+#     0 embed.weight [V,H] f32          1 transformer.norm.weight [H] f32    2 zeros [H] (the final norm has no bias)
+#     per layer l, base = 3 + 10*l, prefix transformer.blocks.l.:
+#       +0 attn.layernorm_qkv.0.weight  +1 .bias       (f32 [H]: LayerNorm before attention)
+#       +2 attn.layernorm_qkv.1.weight [3H,H] 16-bit (rows: q | k | v)
+#       +3 attn.q_ln.weight  +4 attn.k_ln.weight        (f32 [H]: LayerNorm over the whole q / k row, no bias)
+#       +5 attn.out_proj.weight [H,H] 16-bit / s
+#       +6 ffn.0.weight  +7 ffn.0.bias                  (f32 [H]: LayerNorm before the FFN)
+#       +8 ffn.1.weight [2I,H] 16-bit: rows [0,I) gate (silu), [I,2I) up, interleaved as interleave_gate_up
+#       +9 ffn.3.weight [H,I] 16-bit / s
+#
+# s = sqrt(L / 36) is the blocks' residual scale (x + f(x) / s); it is folded into out_proj and ffn.3 in fp32 before
+# the storage rounding (1 for esmc-600m: those weights are untouched).  head_dim is 64, eps 1e-5, rotary base 10000,
+# halves convention; none of these is visible in the weights.
+
+ESMC_HEAD_DIM = 64
+ESMC_EPS = 1e-5
+ESMC_MAX_POS = 2048      # the reference's tokenizer.model_max_length (distllm/embed/encoders/esmc.py:82)
+ESMC_LAYER_KEYS = (
+    ('attn.layernorm_qkv.0.weight', 'H'), ('attn.layernorm_qkv.0.bias', 'H'), ('attn.layernorm_qkv.1.weight', '3H,H'),
+    ('attn.q_ln.weight', 'H'), ('attn.k_ln.weight', 'H'), ('attn.out_proj.weight', 'H,H'),
+    ('ffn.0.weight', 'H'), ('ffn.0.bias', 'H'), ('ffn.1.weight', '2I,H'), ('ffn.3.weight', 'H,I'),
+)
+
+
+class EsmcConfig(NamedTuple):
+    """The shape of an ESM C checkpoint, read from its tensor shapes (:func:`esmc_config`)."""
+
+    hidden_size: int
+    num_hidden_layers: int
+    intermediate_size: int
+    vocab_size: int
+    max_position_embeddings: int = ESMC_MAX_POS
+
+
+def esmc_residual_scale(num_layers: int) -> float:
+    """s = sqrt(L / 36) of esm/layers/blocks.py: each block adds its attention and FFN outputs divided by s."""
+    return (num_layers / 36) ** 0.5
+
+
+def esmc_config(state_dict: Mapping[str, torch.Tensor]) -> EsmcConfig:
+    """Shape inference and validation of an ESM C state dict on tensor shapes alone (nothing moves to a device).
+    Every expected key must be there with its shape; any other key except ``sequence_head.*`` (the LM head, never
+    used) is an error that names it."""
+    shapes = {k: tuple(v.shape) for k, v in state_dict.items() if not k.startswith('sequence_head.')}
+    if 'embed.weight' not in shapes or len(shapes['embed.weight']) != 2:
+        raise ValueError('ESMC checkpoint: no embed.weight [V, H]')
+    v, h = shapes['embed.weight']
+    layers = 0
+    while f'transformer.blocks.{layers}.attn.layernorm_qkv.1.weight' in shapes:
+        layers += 1
+    if layers == 0:
+        raise ValueError('ESMC checkpoint: no transformer.blocks.0')
+    w1 = shapes.get('transformer.blocks.0.ffn.1.weight', ())
+    if len(w1) != 2 or w1[0] % 2:
+        raise ValueError(f'ESMC checkpoint: transformer.blocks.0.ffn.1.weight has shape {w1}, expected [2I, {h}]')
+    i = w1[0] // 2
+    dims = {'H': h, '3H': 3 * h, '2I': 2 * i, 'I': i}
+    want = {'embed.weight': (v, h), 'transformer.norm.weight': (h,)}
+    for layer in range(layers):
+        for key, shape in ESMC_LAYER_KEYS:
+            want[f'transformer.blocks.{layer}.{key}'] = tuple(dims[d] for d in shape.split(','))
+    unexpected = sorted(set(shapes) - set(want))
+    if unexpected:
+        raise ValueError(f'ESMC checkpoint: unexpected keys {unexpected[:8]} (built: the esm package ESMC layout '
+                         f'without Linear biases and with full-width q_ln / k_ln)')
+    for key, shape in want.items():
+        if key not in shapes:
+            raise ValueError(f'ESMC checkpoint: missing {key}')
+        if shapes[key] != shape:
+            raise ValueError(f'ESMC checkpoint: {key} has shape {list(shapes[key])}, expected {list(shape)}')
+    return EsmcConfig(hidden_size=h, num_hidden_layers=layers, intermediate_size=i, vocab_size=v)
+
+
+def esmc_desc(config: EsmcConfig) -> _native.ModelDesc:
+    """Translate an :class:`EsmcConfig` into the C ``B2EModelDesc`` (b2e_check_model decides what is built)."""
+    h = config.hidden_size
+    return _native.ModelDesc(
+        arch=_native.ARCH_ESMC,
+        num_layers=config.num_hidden_layers,
+        hidden=h,
+        heads=h // ESMC_HEAD_DIM,
+        kv_heads=h // ESMC_HEAD_DIM,
+        head_dim=ESMC_HEAD_DIM,
+        intermediate=config.intermediate_size,
+        vocab=config.vocab_size,
+        max_pos=config.max_position_embeddings,
+        type_vocab=0,
+        eps=ESMC_EPS,
+        rope_theta=10000.0,
+        sliding_window=0,
+        reserved=0,
+    )
+
+
+def esmc_weight_list(
+    state_dict: Mapping[str, torch.Tensor],
+    num_layers: int,
+    device: torch.device,
+    dtype: torch.dtype = torch.float16,
+    matrix: Callable[[torch.Tensor], Matrix] | None = None,
+) -> list:
+    """ESM C state dict -> contiguous device tensors in ABI order, with 1/s folded into out_proj and ffn.3."""
+    sd = state_dict
+    b16 = matrix or storage_matrix(device, dtype)
+    s = esmc_residual_scale(num_layers)
+
+    def f32(key: str) -> torch.Tensor:
+        return sd[key].detach().to(device=device, dtype=torch.float32).contiguous()
+
+    def scaled(key: str) -> Matrix:
+        w = sd[key].detach().to(device=device, dtype=torch.float32)
+        return b16(w if s == 1.0 else w / s)
+
+    norm = f32('transformer.norm.weight')
+    out = [f32('embed.weight'), norm, torch.zeros_like(norm)]
+    for layer in range(num_layers):
+        p = f'transformer.blocks.{layer}.'
+        w1 = b16(sd[p + 'ffn.1.weight'])
+        i = sd[p + 'ffn.1.weight'].shape[0] // 2
+        out += [
+            f32(p + 'attn.layernorm_qkv.0.weight'), f32(p + 'attn.layernorm_qkv.0.bias'),
+            b16(sd[p + 'attn.layernorm_qkv.1.weight']),
+            f32(p + 'attn.q_ln.weight'), f32(p + 'attn.k_ln.weight'),
+            scaled(p + 'attn.out_proj.weight'),
+            f32(p + 'ffn.0.weight'), f32(p + 'ffn.0.bias'),
+            interleave_gate_up(row_slice(w1, 0, i), row_slice(w1, i, 2 * i)),
+            scaled(p + 'ffn.3.weight'),
+        ]
+    return out
+
+
+def random_esmc_state_dict(hidden: int, num_layers: int, intermediate: int, seed: int = 0,
+                           device: torch.device | str = 'cpu', std: float = 0.02,
+                           vocab: int = 64) -> dict[str, torch.Tensor]:
+    """Seeded random ESM C weights with the checkpoint's key names and shapes, including a small ``sequence_head``
+    (which the loader skips).  Every norm gain is 1 + N(0, std) and every norm bias N(0, std), so that a missing or
+    swapped norm parameter changes the result."""
+    gen = torch.Generator(device=device)
+    gen.manual_seed(seed)
+    h, i = hidden, intermediate
+
+    def normal(*shape: int) -> torch.Tensor:
+        return torch.randn(*shape, generator=gen, device=device, dtype=torch.float32) * std
+
+    sd: dict[str, torch.Tensor] = {'embed.weight': normal(vocab, h), 'transformer.norm.weight': 1.0 + normal(h)}
+    for layer in range(num_layers):
+        p = f'transformer.blocks.{layer}.'
+        sd[p + 'attn.layernorm_qkv.0.weight'] = 1.0 + normal(h)
+        sd[p + 'attn.layernorm_qkv.0.bias'] = normal(h)
+        sd[p + 'attn.layernorm_qkv.1.weight'] = normal(3 * h, h)
+        sd[p + 'attn.q_ln.weight'] = 1.0 + normal(h)
+        sd[p + 'attn.k_ln.weight'] = 1.0 + normal(h)
+        sd[p + 'attn.out_proj.weight'] = normal(h, h)
+        sd[p + 'ffn.0.weight'] = 1.0 + normal(h)
+        sd[p + 'ffn.0.bias'] = normal(h)
+        sd[p + 'ffn.1.weight'] = normal(2 * i, h)
+        sd[p + 'ffn.3.weight'] = normal(h, i)
+    sd['sequence_head.0.weight'] = normal(h, h)
+    sd['sequence_head.0.bias'] = normal(h)
+    sd['sequence_head.3.weight'] = normal(vocab, h)
+    return sd

@@ -89,12 +89,18 @@ class ExactIndex:
             self.embedding_size = matrix.shape[1]
             return
         dtype = torch.float32 if self.config.corpus_dtype == 'float32' else torch.bfloat16
-        self.corpus = matrix.to(device=dev, dtype=dtype).contiguous()
+        self.corpus = matrix.to(device=dev, dtype=dtype)
+        # the scans read one 16-byte vector per lane: rows are zero-padded to a multiple of 128 (float32) or 256
+        # (bfloat16) columns (esmc-300m's 960), and queries alike in search; zeros add nothing to any inner product
+        pad = -matrix.shape[1] % (128 if dtype == torch.float32 else 256)
+        if pad:
+            self.corpus = torch.nn.functional.pad(self.corpus, (0, pad))
+        self.corpus = self.corpus.contiguous()
         self.embedding_size = matrix.shape[1]
         # bound of the row norms: sizes the TF32 margin of the tensor-core scan (b2e_topk_ip_tc).  Computed once
-        # here, a hair above the measured maximum; None (bf16 corpus, odd widths) keeps the CUDA-core scan.
+        # here, a hair above the measured maximum; None (bf16 corpus) keeps the CUDA-core scan.
         self.max_norm = None
-        if dtype == torch.float32 and matrix.shape[0] > 0 and matrix.shape[1] % 128 == 0:
+        if dtype == torch.float32 and matrix.shape[0] > 0:
             self.max_norm = _native.max_row_norm(self.corpus) * 1.0001
 
     def __len__(self) -> int:
@@ -121,6 +127,8 @@ class ExactIndex:
                 raise _native.NativeError('ubinary search: more rows tie at the threshold Hamming distance than '
                                           'the candidate buffer holds (duplicate corpus rows?)')
         else:
+            if queries.shape[-1] == self.embedding_size < self.corpus.shape[1]:
+                queries = torch.nn.functional.pad(queries, (0, self.corpus.shape[1] - queries.shape[-1])).contiguous()
             scores, indices = _native.topk_ip(queries, self.corpus, top_k, max_norm=self.max_norm)
         scores, indices = scores.cpu(), indices.cpu()
         total_scores, total_indices = [], []

@@ -15,6 +15,8 @@
  *                           HF Qwen3Model.forward, transformers/models/qwen3/modeling_qwen3.py)
  *                           and distllm/embed/encoders/esm2.py:109-134 (Esm2Encoder.encode -> HF
  *                           EsmForMaskedLM, transformers/models/esm/modeling_esm.py:189-516)
+ *                           and distllm/embed/encoders/esmc.py:115-134 (EsmCambrianEncoder.encode -> the esm
+ *                           package's ESMC.forward, esm/models/esmc.py)
  *   b2e_encode_pooled       distllm/embed/embedders/full_sequence.py:59-69 (encode + pool + normalize)
  *   b2e_embed_host          distllm/embed/embedders/full_sequence.py:57-78 (the whole batch loop,
  *                           host buffers in / host matrix out)
@@ -25,7 +27,8 @@
  *   b2e_topk_ip / b2e_topk_ip_tc / b2e_max_row_norm
  *                           distllm/rag/search.py:280-336 (exact float32 search of the query path)
  *   b2e_gemm_h16 / b2e_attention_d64 / b2e_attention_d32 / b2e_attention_causal_d128 / b2e_qk_norm_rope /
- *   b2e_layernorm:          the building blocks, exported so the parity tests can pin each kernel separately.
+ *   b2e_qk_layernorm_rope / b2e_layernorm:
+ *                           the building blocks, exported so the parity tests can pin each kernel separately.
  */
 #ifndef B2E_H_
 #define B2E_H_
@@ -46,7 +49,14 @@ enum {
   B2E_ERR_NO_DEVICE = 4     /* no sm_90 device: there is no CPU fallback */
 };
 
-enum { B2E_ARCH_BERT = 0, B2E_ARCH_ESM2 = 1, B2E_ARCH_MISTRAL = 2, B2E_ARCH_MODERNBERT = 3, B2E_ARCH_QWEN3 = 4 };
+enum {
+  B2E_ARCH_BERT = 0,
+  B2E_ARCH_ESM2 = 1,
+  B2E_ARCH_MISTRAL = 2,
+  B2E_ARCH_MODERNBERT = 3,
+  B2E_ARCH_QWEN3 = 4,
+  B2E_ARCH_ESMC = 5
+};
 enum { B2E_DTYPE_F32 = 0, B2E_DTYPE_BF16 = 1, B2E_DTYPE_F16 = 2 };
 enum {
   B2E_POOL_MEAN_REF = 0,     /* mean.py semantics incl. the cross-row end-token quirk (mean.py:36) */
@@ -109,13 +119,18 @@ const char* b2e_last_error(void);
  * biases) Wi is ONE matrix with its input / gate halves interleaved in blocks of 64 rows (B2E_EPI_GEGLU),
  * absent norm biases are passed as zero vectors, token_type_ids are ignored.  B2E_ARCH_QWEN3 is B2E_ARCH_MISTRAL
  * with a per-head RMSNorm of every q and k head (over head_dim 128, epsilon desc.eps) before the rotary embedding;
- * desc.sliding_window must be 0. */
+ * desc.sliding_window must be 0.  B2E_ARCH_ESMC (ESM C: 3 + 10*L): 0 embed, 1/2 final LayerNorm g/b (the bias a
+ * zero vector); per layer ln_qkv g/b, Wqkv, q_ln, k_ln (fp32 [H]: a LayerNorm over the whole q / k row, no bias),
+ * Wo, ffn LayerNorm g/b, W1 (gate/up interleaved, B2E_EPI_SWIGLU), W2; no Linear biases.  The rotary base is
+ * desc.rope_theta; the residual scale of the checkpoint is expected folded into Wo and W2; token_type_ids are
+ * ignored. */
 int b2e_num_weights(const B2EModelDesc* desc);
 /* Shape validation only (no device, no weights): 0 when b2e_encoder_create would accept `desc`,
  * else the error it would fail with.  BERT / ESM-2: head_dim 64 or 32, heads*head_dim == H, H in 256 x
  * {1,2,3,4,5,8,10,16}, 384 or 640 (all-MiniLM-L6-v2, bge-small-en-v1.5, e5-small-v2: 384 = 12 x 32; esm2_t30_150M:
  * 640 = 20 x 32), I % 128 == 0; Mistral and Qwen3: head_dim 128 (see above); Mistral, Qwen3 and ModernBERT: H a
- * multiple of 256 (heads*head_dim may differ from H for Mistral and Qwen3).
+ * multiple of 256 (heads*head_dim may differ from H for Mistral and Qwen3); ESMC: head_dim 64, heads*64 == H, H 960
+ * (esmc-300m) or 1152 (esmc-600m), I % 128 == 0.
  * Call it BEFORE uploading weights (distllm/embed/encoders/auto.py:59-63 loads the checkpoint unconditionally). */
 int b2e_check_model(const B2EModelDesc* desc);
 int b2e_encoder_create(const B2EModelDesc* desc, const void* const* weights, int n_weights,
@@ -216,6 +231,13 @@ int b2e_attention_causal_d128(const void* qkv, const int64_t* attention_mask, vo
 int b2e_qk_norm_rope(void* qkv, const float* q_gamma, const float* k_gamma, const float* cos_t, const float* sin_t,
                      int T, int S, int heads, int kv_heads, float eps, const int* t_real /* nullable */,
                      const int* tok_src /* nullable */, void* stream);
+/* ESMC's q/k step, in place on qkv [T, 3H] (columns q | k | v, H = 960 or 1152): the q row x (H columns) becomes
+ * rotary(q_gamma * (x - mean) * rsqrt(var + eps)), a LayerNorm over the whole row without bias, the k row the same
+ * with k_gamma (fp32 [H] each), the rotation per 64-wide head in the halves convention; v is untouched.  cos_t /
+ * sin_t are [S, 32] fp32, positions and t_real / tok_src as in b2e_qk_norm_rope. */
+int b2e_qk_layernorm_rope(void* qkv, const float* q_gamma, const float* k_gamma, const float* cos_t,
+                          const float* sin_t, int T, int S, int H, float eps, const int* t_real /* nullable */,
+                          const int* tok_src /* nullable */, void* stream);
 /* Exact inner-product top-k over a device-resident embedding matrix (the retrieval query path,
  * distllm/rag/search.py:280-336: faiss IndexFlatIP through semantic_search_faiss, float32/exact).
  * queries [Q,H] f32, corpus [N,H] F32 or BF16 (both row-major on the device), 1 <= k <= 256,

@@ -5,7 +5,7 @@ For each encoder family at its BASELINE shape, on N(0, 0.02) weights and on outl
 attended token's hidden state is compared with the oracle's state at the same depth: min / mean cosine per
 depth, plus the pooled embedding's cosine at full depth.  Writes a markdown table per case.
 
-usage: drift_report.py [out.md] [families: bert,esm,mistral,qwen3]
+usage: drift_report.py [out.md] [families: bert,esm,mistral,qwen3,esmc]
 """
 import sys
 import time
@@ -182,6 +182,41 @@ def run_qwen3(lines):
         torch.cuda.empty_cache()
 
 
+def run_esmc(lines):
+    """esmc-600m shape (36 layers, H 1152, 18 heads x 64, I 3072) at S = 2048, the longest input the tokenizer
+    allows, in BOTH storage builds: the measurement behind _native._STORAGE_BY_ARCH['esmc']."""
+    from distllm_b200.embed.encoders import weights as W
+    from distllm_b200.embed.encoders.native import NativeEsmcEncoder
+    from tools.oracle_esmc import esmc_forward
+
+    dev = torch.device('cuda:0')
+    g = torch.Generator().manual_seed(25)
+    b, s = 2, 2048
+    lens = torch.tensor([2048, 1400])
+    ids = torch.randint(4, 24, (b, s), generator=g)
+    ids[:, 0] = 0
+    ids[torch.arange(b), lens - 1] = 2
+    mask = (torch.arange(s)[None] < lens[:, None]).long()
+    ids[mask == 0] = 1
+    for w in ('normal', 'outliers'):
+        sd = W.random_esmc_state_dict(1152, 36, 3072, seed=6, device=dev)
+        if w == 'outliers':
+            add_outliers(sd, 'esmc', seed=4)
+        t0 = time.time()
+        states = [t.cpu() for t in esmc_forward(sd, ids.to(dev), mask.to(dev), every_depth=True)]
+        print(f'esmc oracle {time.time() - t0:.1f} s', flush=True)
+        ref_pool = opool.average_pool(states[-1], mask.clone()).numpy()
+        for storage in ('f16', 'bf16'):
+            enc = NativeEsmcEncoder(W.esmc_config(sd), sd, device=dev, storage=storage)
+            report(f'esmc-600m shape, 36 layers, S=2048 (rows of 2048 and 1400 tokens), {w} weights, {storage} build '
+                   f'(mean pooler)', enc, ids, mask, None, states, ref_pool, nv.POOL_MEAN_REF, lines)
+            enc.close()
+            del enc
+            torch.cuda.empty_cache()
+        del sd, states
+        torch.cuda.empty_cache()
+
+
 if __name__ == '__main__':
     out = Path(sys.argv[1]) if len(sys.argv) > 1 else Path('gpurun_out/drift_report.md')
     fams = (sys.argv[2] if len(sys.argv) > 2 else 'bert,esm,mistral').split(',')
@@ -190,7 +225,8 @@ if __name__ == '__main__':
              'Model truncated to l layers on both sides (BERT: hidden_states[l]; ESM-2 / Mistral: final norm of the '
              'residual stream after l layers); cosine per attended token.  GEMMs multiply in bf16 with fp32 '
              'accumulation; norm statistics, softmax and pooling are fp32.']
-    for fam, fn in (('bert', run_bert), ('esm', run_esm), ('mistral', run_mistral), ('qwen3', run_qwen3)):
+    for fam, fn in (('bert', run_bert), ('esm', run_esm), ('mistral', run_mistral), ('qwen3', run_qwen3),
+                    ('esmc', run_esmc)):
         if fam in fams:
             fn(lines)
             out.parent.mkdir(parents=True, exist_ok=True)

@@ -103,7 +103,12 @@ _OUT_ROWS = {
     'mistral': ('self_attn.o_proj.weight', 'mlp.down_proj.weight'),
     'qwen3': ('self_attn.o_proj.weight', 'mlp.down_proj.weight'),
     'modernbert': ('attn.Wo.weight', 'mlp.Wo.weight'),
+    'esmc': ('attn.out_proj.weight', 'ffn.3.weight'),
 }
+# ESM C's block norms and its full-width q_ln / k_ln (names the hidden-channel loop does not match)
+_ESMC_NORMS = ('attn.layernorm_qkv.0.weight', 'ffn.0.weight')
+_ESMC_BIASES = ('attn.layernorm_qkv.0.bias', 'ffn.0.bias')
+_ESMC_QK = ('attn.q_ln.weight', 'attn.k_ln.weight')
 
 
 def add_outliers(state_dict: dict, family: str, seed: int = 0, n_massive: int = 4, scale: float = 50.0,
@@ -124,7 +129,9 @@ def add_outliers(state_dict: dict, family: str, seed: int = 0, n_massive: int = 
 
     Qwen3's per-head q_norm / k_norm gains ([head_dim], applied right before the attention logits) take no part
     in the hidden-channel draws above; for the same reason they get log-uniform gains in ``gain_range`` only,
-    from a generator of their own, so the other families' weights are drawn exactly as before."""
+    from a generator of their own, so the other families' weights are drawn exactly as before.  ESM C's block norms
+    (massive / loud channels as above), their biases and its q_ln / k_ln gains (log-uniform only, for the same reason)
+    come from that second generator too."""
     g = torch.Generator().manual_seed(seed)
     out_names = _OUT_ROWS[family]
     hidden = next(v.shape[0] for k, v in state_dict.items() if k.endswith(out_names[0]))
@@ -152,4 +159,15 @@ def add_outliers(state_dict: dict, family: str, seed: int = 0, n_massive: int = 
             if name.endswith(head_norms):
                 gain = torch.exp(torch.rand(t.shape, generator=g_head) * (hi - lo) + lo)
                 t.copy_(gain.to(device=t.device, dtype=t.dtype))
+    if family == 'esmc':
+        g_esmc = torch.Generator().manual_seed(seed + 1)
+        for name, t in state_dict.items():
+            if name.endswith(_ESMC_NORMS + _ESMC_QK):
+                gain = torch.exp(torch.rand(t.shape, generator=g_esmc) * (hi - lo) + lo)
+                if name.endswith(_ESMC_NORMS):
+                    gain[massive] = massive_gain
+                    gain[loud] = loud_gain
+                t.copy_(gain.to(device=t.device, dtype=t.dtype))
+            elif name.endswith(_ESMC_BIASES):
+                t.copy_((0.5 * torch.randn(t.shape, generator=g_esmc)).to(device=t.device, dtype=t.dtype))
     return state_dict
