@@ -85,6 +85,9 @@ EXPORTS = (
     'b2e_topk_ip',
     'b2e_topk_ip_tc',
     'b2e_max_row_norm',
+    'b2e_topk_l2',
+    'b2e_topk_l2_tc',
+    'b2e_row_norms',
     'b2e_pack_ubinary',
     'b2e_search_ubinary',
     'b2e_layernorm',
@@ -200,6 +203,12 @@ def _declare(lib: C.CDLL) -> None:
     lib.b2e_topk_ip_tc.argtypes = [vp, i32, vp, i64, i32, i32, C.c_float, vp, vp, vp]
     lib.b2e_max_row_norm.restype = i32
     lib.b2e_max_row_norm.argtypes = [vp, i64, i32, C.POINTER(C.c_float), vp]
+    lib.b2e_topk_l2.restype = i32
+    lib.b2e_topk_l2.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, vp]
+    lib.b2e_topk_l2_tc.restype = i32
+    lib.b2e_topk_l2_tc.argtypes = [vp, i32, vp, vp, i64, i32, i32, C.c_float, vp, vp, vp]
+    lib.b2e_row_norms.restype = i32
+    lib.b2e_row_norms.argtypes = [vp, i64, i32, vp, C.POINTER(C.c_float), vp]
     lib.b2e_pack_ubinary.restype = i32
     lib.b2e_pack_ubinary.argtypes = [vp, i64, i32, vp, vp]
     lib.b2e_search_ubinary.restype = i32
@@ -582,8 +591,54 @@ def max_row_norm(matrix: torch.Tensor) -> float:
     return float(out.value)
 
 
+def topk_l2(queries: torch.Tensor, corpus: torch.Tensor, k: int, norms: torch.Tensor | None = None,
+            max_norm: float | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """Exact squared-L2 top-k: queries [Q,H] f32, corpus [N,H] f32 (CUDA) -> (distances [Q,k] f32, indices [Q,k]
+    i64), ascending squared Euclidean distance, ties by ascending index, +inf / -1 past N.  ``norms`` and
+    ``max_norm`` (both from :func:`row_norms` on this corpus) select the tensor-core scan; the results are the
+    same."""
+    lib = load()
+    _cuda_contig(queries, 'queries'), _cuda_contig(corpus, 'corpus')
+    if queries.dtype != torch.float32 or corpus.dtype != torch.float32:
+        raise NativeError('topk_l2 expects float32 queries and corpus')
+    if (norms is None) != (max_norm is None):
+        raise NativeError('topk_l2: pass both norms and max_norm (row_norms) or neither')
+    q, h = queries.shape
+    n = corpus.shape[0]
+    dist = torch.empty((q, k), dtype=torch.float32, device=queries.device)
+    indices = torch.empty((q, k), dtype=torch.int64, device=queries.device)
+    with torch.cuda.device(queries.device):
+        if norms is not None:
+            _cuda_contig(norms, 'norms')
+            if norms.dtype != torch.float32 or norms.shape != (n,):
+                raise NativeError(f'norms must be float32 [{n}]')
+            check(lib.b2e_topk_l2_tc(queries.data_ptr(), q, corpus.data_ptr(), norms.data_ptr(), n, h, k,
+                                     float(max_norm), dist.data_ptr(), indices.data_ptr(),
+                                     stream_ptr(queries.device)))
+        else:
+            check(lib.b2e_topk_l2(queries.data_ptr(), q, corpus.data_ptr(), n, h, k, dist.data_ptr(),
+                                  indices.data_ptr(), stream_ptr(queries.device)))
+    return dist, indices
+
+
+def row_norms(matrix: torch.Tensor) -> tuple[torch.Tensor, float]:
+    """(squared Euclidean norm of every row, fp32 [N] on the device; largest row norm) of a float32 CUDA matrix:
+    the index-build step of the tensor-core L2 search."""
+    lib = load()
+    _cuda_contig(matrix, 'matrix')
+    if matrix.dtype != torch.float32:
+        raise NativeError('row_norms expects float32')
+    norms = torch.empty(matrix.shape[0], dtype=torch.float32, device=matrix.device)
+    out = C.c_float(0.0)
+    with torch.cuda.device(matrix.device):
+        check(lib.b2e_row_norms(matrix.data_ptr(), matrix.shape[0], matrix.shape[1], norms.data_ptr(), C.byref(out),
+                                stream_ptr(matrix.device)))
+    return norms, float(out.value)
+
+
 def topk_tc_fell_back() -> bool:
-    """Whether this thread's last tensor-core search had to redo the call with the exact scan (debug hook)."""
+    """Whether this thread's last tensor-core search (inner product or L2) had to redo the call with the exact scan
+    (debug hook)."""
     lib = load()
     out = C.c_int(0)
     lib.b2e_debug_topk_tc_fell_back.argtypes = [C.POINTER(C.c_int)]

@@ -2007,9 +2007,9 @@ struct TopkScratch : DeviceScratch {
 };
 thread_local TopkScratch g_topk_scratch;
 
-template <typename T, int QT, int ROWS, int VMAX>
+template <typename T, int QT, int ROWS, int VMAX, bool L2>
 int launch_topk_cfg(const float* queries, int Q, const T* corpus, int64_t N, int H, int k, float* out_score,
-                    int64_t* out_index, int sms, cudaStream_t st, const int* run_flag = nullptr) {
+                    int64_t* out_index, int sms, cudaStream_t st, const int* run_flag) {
   // queries per pass: bounded by QT and by ~160 KiB of shared memory for the query tile
   int qt = QT;
   while (qt > 1 && (size_t)qt * H * 4 > 160 * 1024) qt >>= 1;
@@ -2018,7 +2018,7 @@ int launch_topk_cfg(const float* queries, int Q, const T* corpus, int64_t N, int
   const int grid = (int)(want < (long long)2 * sms ? (want > 0 ? want : 1) : (long long)2 * sms);
   int rc;
   if ((rc = g_topk_scratch.ensure((size_t)grid * qt * k))) return rc;
-  auto kern = topk_scan_kernel<T, QT, ROWS, VMAX>;
+  auto kern = topk_scan_kernel<T, QT, ROWS, VMAX, L2>;
   const size_t smem_max = (size_t)qt * H * 4 + (size_t)qt * k * 12 + 8 + (size_t)qt * 12;
   // (k varies between calls: always set the attribute to this call's worst case)
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
@@ -2027,7 +2027,7 @@ int launch_topk_cfg(const float* queries, int Q, const T* corpus, int64_t N, int
     const size_t smem = (size_t)nq * H * 4 + (size_t)nq * k * 12 + 8 + (size_t)nq * 12;
     kern<<<grid, TOPK_THREADS, smem, st>>>(queries + (size_t)q0 * H, corpus, nq, (long long)N, H, k,
                                            g_topk_scratch.score, g_topk_scratch.index, run_flag);
-    topk_merge_kernel<<<nq, TOPK_THREADS, 0, st>>>(g_topk_scratch.score, g_topk_scratch.index, grid, nq,
+    topk_merge_kernel<L2><<<nq, TOPK_THREADS, 0, st>>>(g_topk_scratch.score, g_topk_scratch.index, grid, nq,
                                                    k, out_score + (size_t)q0 * k,
                                                    out_index + (size_t)q0 * k, k, run_flag);
   }
@@ -2035,14 +2035,15 @@ int launch_topk_cfg(const float* queries, int Q, const T* corpus, int64_t N, int
   return B2E_OK;
 }
 
-// one to four queries: the narrow, deeper scan; more: 16 queries per pass
-template <typename T, int VWIDE, int VNARROW>
+// one to four queries: the narrow, deeper scan; more: 16 queries per pass.  L2: squared distances (float32 only)
+template <typename T, int VWIDE, int VNARROW, bool L2 = false>
 int launch_topk(const float* queries, int Q, const T* corpus, int64_t N, int H, int k, float* out_score,
                 int64_t* out_index, int sms, cudaStream_t st, const int* run_flag = nullptr) {
   if (Q <= 4)
-    return launch_topk_cfg<T, 4, 8, VNARROW>(queries, Q, corpus, N, H, k, out_score, out_index, sms, st, run_flag);
-  return launch_topk_cfg<T, TOPK_QT, 4, VWIDE>(queries, Q, corpus, N, H, k, out_score, out_index, sms, st,
-                                               run_flag);
+    return launch_topk_cfg<T, 4, 8, VNARROW, L2>(queries, Q, corpus, N, H, k, out_score, out_index, sms, st,
+                                                 run_flag);
+  return launch_topk_cfg<T, TOPK_QT, 4, VWIDE, L2>(queries, Q, corpus, N, H, k, out_score, out_index, sms, st,
+                                                   run_flag);
 }
 
 // ---- tensor-core fast path (topk_tc.cuh)
@@ -2094,10 +2095,22 @@ int b2e_topk_ip(const float* queries, int Q, const void* corpus, int corpus_dtyp
   return fail(B2E_ERR_INVALID, "topk: corpus dtype %d (F32 or BF16)", corpus_dtype);
 }
 
-// largest Euclidean row norm of a float32 matrix (synchronises the stream: an index-build step, not a query step)
-int b2e_max_row_norm(const float* x, int64_t N, int H, float* out_host, void* stream) {
-  if (!x || !out_host) return fail(B2E_ERR_INVALID, "null tensor pointer");
-  if (N <= 0 || H <= 0 || H % 4 != 0) return fail(B2E_ERR_INVALID, "max_row_norm: N=%lld H=%d", (long long)N, H);
+int b2e_topk_l2(const float* queries, int Q, const float* corpus, int64_t N, int H, int k, float* out_dist,
+                int64_t* out_indices, void* stream) {
+  if (!queries || !corpus || !out_dist || !out_indices) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (Q <= 0 || N <= 0) return fail(B2E_ERR_INVALID, "topk_l2: empty problem Q=%d N=%lld", Q, (long long)N);
+  if (k <= 0 || k > TOPK_MAX_K) return fail(B2E_ERR_INVALID, "topk_l2: k=%d must be in [1, %d]", k, TOPK_MAX_K);
+  if (H % 128 != 0 || H > 8192) return fail(B2E_ERR_INVALID, "topk_l2: H=%d must be a multiple of 128 (<= 8192)", H);
+  int rc;
+  DeviceInfo info;
+  if ((rc = current_device_info(&info))) return rc;
+  return launch_topk<float, 6, 3, true>(queries, Q, corpus, N, H, k, out_dist, out_indices, info.sms,
+                                        (cudaStream_t)stream);
+}
+
+int b2e_row_norms(const float* x, int64_t N, int H, float* out_norm2, float* out_max_host, void* stream) {
+  if (!x || !out_max_host) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (N <= 0 || H <= 0 || H % 4 != 0) return fail(B2E_ERR_INVALID, "row_norms: N=%lld H=%d", (long long)N, H);
   int rc;
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
@@ -2105,23 +2118,26 @@ int b2e_max_row_norm(const float* x, int64_t N, int H, float* out_host, void* st
   if ((rc = sc.ensure(TC_ROWS, 128))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   CUDA_TRY(cudaMemsetAsync(sc.norm2, 0, sizeof(float), st));
-  max_row_norm2_kernel<<<info.sms * 4, 256, 0, st>>>(x, (long long)N, H, sc.norm2);
+  row_norm2_kernel<<<info.sms * 4, 256, 0, st>>>(x, (long long)N, H, out_norm2, sc.norm2);
   float n2 = 0.0f;
   CUDA_TRY(cudaMemcpyAsync(&n2, sc.norm2, sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  *out_host = sqrtf(n2);
+  *out_max_host = sqrtf(n2);
   return B2E_OK;
 }
 
-// Exact inner-product top-k with the scan on the tensor cores (topk_tc.cuh).  corpus_max_norm bounds the Euclidean
-// norm of every corpus row (b2e_max_row_norm; 1 for normalised embeddings): it sizes the TF32 error margin.
-// Same results as b2e_topk_ip; small problems and anything the fast path cannot take go there directly.
-int b2e_topk_ip_tc(const float* queries, int Q, const float* corpus, int64_t N, int H, int k,
+// largest Euclidean row norm of a float32 matrix (synchronises the stream: an index-build step, not a query step)
+int b2e_max_row_norm(const float* x, int64_t N, int H, float* out_host, void* stream) {
+  return b2e_row_norms(x, N, H, nullptr, out_host, stream);
+}
+
+extern "C++" {
+namespace {
+// The tensor-core search (topk_tc.cuh) for both metrics.  Inner product: norm2 unused, shift 0.  L2: norm2 [N] from
+// b2e_row_norms, shift = corpus_max_norm^2 / 2 (the histogram's range below -r).
+template <bool L2>
+int launch_topk_tc(const float* queries, int Q, const float* corpus, const float* norm2, int64_t N, int H, int k,
                    float corpus_max_norm, float* out_scores, int64_t* out_indices, void* stream) {
-  if (!queries || !corpus || !out_scores || !out_indices) return fail(B2E_ERR_INVALID, "null tensor pointer");
-  const bool fast = N >= 32768 && N < ((int64_t)1 << 31) - TC_ROWS && H % 128 == 0 && H <= 8192 && k > 0 && k <= TOPK_MAX_K &&
-                    corpus_max_norm > 0.0f && corpus_max_norm < 1e30f && Q > 0;
-  if (!fast) return b2e_topk_ip(queries, Q, corpus, B2E_DTYPE_F32, N, H, k, out_scores, out_indices, stream);
   int rc;
   DeviceInfo info;
   if ((rc = current_device_info(&info))) return rc;
@@ -2133,32 +2149,66 @@ int b2e_topk_ip_tc(const float* queries, int Q, const float* corpus, int64_t N, 
   if ((rc = make_tmap_f32(&tm_c, corpus, (uint64_t)N, (uint64_t)H, TC_ROWS))) return rc;
   if ((rc = make_tmap_f32(&tm_q, sc.qpad, TC_NQ, (uint64_t)H, TC_NQ))) return rc;
   if ((rc = ensure_smem_attr(tf32_scan_kernel, TC_SMEM_BYTES))) return rc;
-  if ((rc = ensure_smem_attr(score_hist_kernel, TC_NQ * TC_BINS * 4))) return rc;
-  if ((rc = ensure_smem_attr(exact_rescore_kernel, TC_MAX_CAND * 8 + 8192 * 4))) return rc;
+  if ((rc = ensure_smem_attr(score_hist_kernel<L2>, TC_NQ * TC_BINS * 4))) return rc;
+  if ((rc = ensure_smem_attr(exact_rescore_kernel<L2>, TC_MAX_CAND * 8 + 8192 * 4))) return rc;
   CUDA_TRY(cudaMemsetAsync(sc.flag, 0, 2 * sizeof(int), st));
   const int grid_scan = tiles < info.sms ? (int)tiles : info.sms;
   const int grid_rows = info.sms * 2;
+  const float shift = L2 ? 0.5f * corpus_max_norm * corpus_max_norm : 0.0f;
   for (int q0 = 0; q0 < Q; q0 += TC_NQ) {
     const int nq = Q - q0 < TC_NQ ? Q - q0 : TC_NQ;
-    tc_prepare_queries_kernel<<<TC_NQ, 256, 0, st>>>(queries + (size_t)q0 * H, nq, H, corpus_max_norm, sc.qpad,
-                                                     sc.meta);
+    tc_prepare_queries_kernel<L2><<<TC_NQ, 256, 0, st>>>(queries + (size_t)q0 * H, nq, H, corpus_max_norm, sc.qpad,
+                                                         sc.meta);
     CUDA_TRY(cudaMemsetAsync(sc.hist, 0, (size_t)TC_NQ * TC_BINS * sizeof(unsigned), st));
     CUDA_TRY(cudaMemsetAsync(sc.n_cand, 0, TC_NQ * sizeof(unsigned), st));
     tf32_scan_kernel<<<grid_scan, TC_THREADS, TC_SMEM_BYTES, st>>>(tm_c, tm_q, sc.scores, tiles, H);
-    score_hist_kernel<<<grid_rows, 512, (size_t)nq * TC_BINS * 4, st>>>(sc.scores, (long long)N, nq, sc.meta,
-                                                                        sc.hist);
-    score_threshold_kernel<<<1, 32 * TC_NQ, 0, st>>>(sc.hist, nq, (long long)N, k, sc.meta);
-    score_select_kernel<<<grid_rows, 512, 0, st>>>(sc.scores, (long long)N, nq, sc.meta, sc.cand, sc.n_cand);
-    exact_rescore_kernel<<<nq, 512, (size_t)TC_MAX_CAND * 8 + (size_t)H * 4, st>>>(
+    score_hist_kernel<L2><<<grid_rows, 512, (size_t)nq * TC_BINS * 4, st>>>(sc.scores, (long long)N, nq, sc.meta,
+                                                                            sc.hist, norm2, shift);
+    score_threshold_kernel<L2><<<1, 32 * TC_NQ, 0, st>>>(sc.hist, nq, (long long)N, k, sc.meta, shift);
+    score_select_kernel<L2><<<grid_rows, 512, 0, st>>>(sc.scores, (long long)N, nq, sc.meta, sc.cand, sc.n_cand,
+                                                       norm2);
+    exact_rescore_kernel<L2><<<nq, 512, (size_t)TC_MAX_CAND * 8 + (size_t)H * 4, st>>>(
         sc.cand, sc.n_cand, sc.meta, queries + (size_t)q0 * H, corpus, H, k, out_scores + (size_t)q0 * k,
         out_indices + (size_t)q0 * k, sc.flag);
   }
   CUDA_TRY(cudaGetLastError());
   // the exact scan redoes the call when a candidate list overflowed; otherwise its kernels return at once
-  return launch_topk<float, 6, 3>(queries, Q, corpus, N, H, k, out_scores, out_indices, info.sms, st, sc.flag);
+  return launch_topk<float, 6, 3, L2>(queries, Q, corpus, N, H, k, out_scores, out_indices, info.sms, st, sc.flag);
 }
 
-// 1 when the last b2e_topk_ip_tc call of this thread had to fall back to the exact scan (synchronises the device)
+// the tensor-core path takes 2^15 <= N < 2^31 - 128 rows; the rest goes to the CUDA-core scan directly
+bool topk_tc_takes(int Q, int64_t N, int H, int k, float corpus_max_norm) {
+  return N >= 32768 && N < ((int64_t)1 << 31) - TC_ROWS && H % 128 == 0 && H <= 8192 && k > 0 && k <= TOPK_MAX_K &&
+         corpus_max_norm > 0.0f && corpus_max_norm < 1e30f && Q > 0;
+}
+}  // namespace
+}  // extern "C++"
+
+// Exact inner-product top-k with the scan on the tensor cores (topk_tc.cuh).  corpus_max_norm bounds the Euclidean
+// norm of every corpus row (b2e_max_row_norm; 1 for normalised embeddings): it sizes the TF32 error margin.
+// Same results as b2e_topk_ip; small problems and anything the fast path cannot take go there directly.
+int b2e_topk_ip_tc(const float* queries, int Q, const float* corpus, int64_t N, int H, int k,
+                   float corpus_max_norm, float* out_scores, int64_t* out_indices, void* stream) {
+  if (!queries || !corpus || !out_scores || !out_indices) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (!topk_tc_takes(Q, N, H, k, corpus_max_norm))
+    return b2e_topk_ip(queries, Q, corpus, B2E_DTYPE_F32, N, H, k, out_scores, out_indices, stream);
+  return launch_topk_tc<false>(queries, Q, corpus, nullptr, N, H, k, corpus_max_norm, out_scores, out_indices,
+                               stream);
+}
+
+// Exact squared-L2 top-k with the scan on the tensor cores: the same scan, ranked on S - |x|^2 / 2 with the stored
+// norms, decided on fp32 distances (topk_tc.cuh).  Same results as b2e_topk_l2.
+int b2e_topk_l2_tc(const float* queries, int Q, const float* corpus, const float* corpus_norm2, int64_t N, int H,
+                   int k, float corpus_max_norm, float* out_dist, int64_t* out_indices, void* stream) {
+  if (!queries || !corpus || !corpus_norm2 || !out_dist || !out_indices)
+    return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (!topk_tc_takes(Q, N, H, k, corpus_max_norm))
+    return b2e_topk_l2(queries, Q, corpus, N, H, k, out_dist, out_indices, stream);
+  return launch_topk_tc<true>(queries, Q, corpus, corpus_norm2, N, H, k, corpus_max_norm, out_dist, out_indices,
+                              stream);
+}
+
+// 1 when the last b2e_topk_ip_tc / b2e_topk_l2_tc call of this thread had to fall back to the exact scan (synchronises the device)
 int b2e_debug_topk_tc_fell_back(int* out) {
   if (!out) return fail(B2E_ERR_INVALID, "null pointer");
   *out = 0;

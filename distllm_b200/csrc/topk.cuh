@@ -10,6 +10,11 @@
 // shared-memory set under a per-query lock (rare after the first few thousand rows).  A second kernel
 // merges the per-CTA sets of one query and sorts the survivors.  Equal scores are resolved by row id at
 // every step, so the result does not depend on the order in which warps and CTAs reach the rows.
+//
+// The L2 instantiation (float32 corpus only: faiss.IndexFlatL2 of distllm/rag/search.py:402-666, FaissIndexV1
+// with metric='l2') accumulates (q_i - x_i)^2 instead of q_i * x_i and offers -D to the same sets, so "higher
+// score, then lower row id" orders rows by ascending squared distance, ties by ascending row id; the merge writes
+// D = -score back out (an empty slot's -inf becomes +inf).
 #pragma once
 
 #include "common.cuh"
@@ -129,6 +134,12 @@ template <> struct TopkVec<float> {
     const float4 w = *reinterpret_cast<const float4*>(q);
     return fmaf(raw.x, w.x, fmaf(raw.y, w.y, fmaf(raw.z, w.z, fmaf(raw.w, w.w, acc))));
   }
+  // acc + sum (q_i - x_i)^2, in the order dot() sums the products
+  __device__ __forceinline__ float sqdist(const float* q, float acc) const {
+    const float4 w = *reinterpret_cast<const float4*>(q);
+    const float dx = w.x - raw.x, dy = w.y - raw.y, dz = w.z - raw.z, dw = w.w - raw.w;
+    return fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, acc))));
+  }
 };
 template <> struct TopkVec<bf16> {
   static constexpr int E = 8;
@@ -145,7 +156,8 @@ template <> struct TopkVec<bf16> {
 };
 
 // shared memory: queries [nq][H] f32 | sets: score [nq][k] f32, index [nq][k] i64, kth/kth_pos/lock [nq]
-template <typename T, int QT, int ROWS, int VMAX>
+// L2: the sets hold -D (squared Euclidean distance), see the file header.
+template <typename T, int QT, int ROWS, int VMAX, bool L2 = false>
 __global__ void __launch_bounds__(TOPK_THREADS)
 topk_scan_kernel(const float* __restrict__ queries,   // [nq, H] (this pass's query tile)
                  const T* __restrict__ corpus,        // [N, H]
@@ -211,7 +223,10 @@ topk_scan_kernel(const float* __restrict__ queries,   // [nq, H] (this pass's qu
             if (v0 + v < nv) {
               const float* w = qs + static_cast<size_t>(q) * H + ((v0 + v) * 32 + lane) * E;
 #pragma unroll
-              for (int r = 0; r < TOPK_ROWS; ++r) acc[q][r] = x[r][v].dot(w, acc[q][r]);
+              for (int r = 0; r < TOPK_ROWS; ++r) {
+                if constexpr (L2) acc[q][r] = x[r][v].sqdist(w, acc[q][r]);
+                else acc[q][r] = x[r][v].dot(w, acc[q][r]);
+              }
             }
           }
         }
@@ -233,6 +248,10 @@ topk_scan_kernel(const float* __restrict__ queries,   // [nq, H] (this pass's qu
         const float send = upper ? v[i] : v[i + half];
         v[i] = keep + __shfl_xor_sync(0xffffffffu, send, bit);
       }
+    }
+    if constexpr (L2) {
+#pragma unroll
+      for (int j = 0; j < PER; ++j) v[j] = -v[j];
     }
     // the few candidates that reach their query's current k-th score are inserted one by one (a score
     // equal to it may still win on the row id: topk_insert decides); the loop body exists once (64 inlined
@@ -263,7 +282,8 @@ topk_scan_kernel(const float* __restrict__ queries,   // [nq, H] (this pass's qu
 }
 
 // One CTA per query: merge `parts` candidate sets of k entries, sort the k survivors by descending
-// score (ties: ascending index), write them out.  Empty slots (index -1) sort last.
+// score (ties: ascending index), write them out (L2: negated, i.e. D ascending).  Empty slots (index -1) sort last.
+template <bool L2 = false>
 __global__ void __launch_bounds__(TOPK_THREADS)
 topk_merge_kernel(const float* __restrict__ part_score, const int64_t* __restrict__ part_index, int parts,
                   int nq, int k, float* __restrict__ out_score, int64_t* __restrict__ out_index,
@@ -318,7 +338,7 @@ topk_merge_kernel(const float* __restrict__ part_score, const int64_t* __restric
     }
   }
   for (int i = threadIdx.x; i < k; i += TOPK_THREADS) {
-    out_score[static_cast<size_t>(q) * out_stride + i] = s_score[i];
+    out_score[static_cast<size_t>(q) * out_stride + i] = L2 ? -s_score[i] : s_score[i];
     out_index[static_cast<size_t>(q) * out_stride + i] = s_index[i];
   }
 }

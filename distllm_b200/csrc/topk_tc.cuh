@@ -20,6 +20,25 @@
 // A query whose candidate list overflows (scores packed closer than eps around the k-th: duplicates, degenerate
 // corpora) raises a device-side flag; the exact FMA scan of topk.cuh then runs for the call (it returns at once
 // when the flag is clear), so the result never depends on the approximation.
+//
+// Squared-L2 search (the <L2 = true> instantiations; faiss.IndexFlatL2 of distllm/rag/search.py:402-666): the
+// scan is the same kernel, S ~ q.x.  Rows are ranked on v = S - n/2, n = fl(|x|^2) from row_norm2_kernel (stored
+// with the index), which orders them like -D because D = |q|^2 + |x|^2 - 2 q.x = |q|^2 - 2 v_exact.  With M >=
+// every |x| (corpus_max_norm) and r = |q| M:
+//   range      v in [-r - M^2/2, r]: the histogram's bins cover that interval instead of [-r, r] (M^2 must bound
+//              every stored n too, so that a k-th value in the lowest bin selects every row and overflows).
+//   eps_S      |S - q.x| <= 1.5 * 2^-9 * r, as above.
+//   norm       n sums H squares in fp32 (depth < H): |n - |x|^2| <= 1.01 H 2^-24 |x|^2 <= H 2^-23 M^2, and v takes
+//              half of it: at most H 2^-24 M^2.
+//   subtract   v = fl(S - n/2) (n/2 is exact): one rounding of a value below r + M^2/2, at most 2^-23 (r + M^2).
+//   distance   the decision computes D~ = fl(sum (q_i - x_i)^2) directly: each difference rounded once, a sum of
+//              non-negative terms of depth < H, so |D~ - D| <= (H + 2) 2^-24 D (1.01) <= H 2^-23 (|q| + M)^2 = e_D.
+// With d = eps_S + H 2^-24 M^2 + 2^-23 (r + M^2) bounding |v - v_exact|: at least `need` rows have v >= edge, so
+// D~ <= |q|^2 - 2 (edge - d) + e_D for each of them, while a row with v < thr has D~ > |q|^2 - 2 (thr + d) - e_D.
+// thr = edge - 2 d - e_D (minus one bin width for the bin arithmetic, as above) therefore leaves out only rows
+// whose computed distance is STRICTLY larger than that of `need` candidates: the decision on D~ (ascending, ties
+// by ascending row id) is the one the exact CUDA-core scan makes.  tc_prepare_queries_kernel<true> stores
+// eps = d + e_D / 2, so the threshold keeps the inner-product form edge - 2 eps - bin.
 #pragma once
 
 #include "common.cuh"
@@ -124,9 +143,11 @@ tf32_scan_kernel(const __grid_constant__ CUtensorMap tm_corpus,    // [N, H] f32
   }
 }
 
-// max over rows of |row|^2 (fp32): what bounds every score by Cauchy-Schwarz.  One warp per row, atomicMax on the
-// bit pattern (non-negative floats order like their integers).  out must be zeroed first.
-__global__ void max_row_norm2_kernel(const float* __restrict__ x, long long N, int H, float* __restrict__ out) {
+// |row|^2 of every row (fp32, a fixed summation order) into norm2 [N] (nullable), and their maximum, what bounds
+// every score by Cauchy-Schwarz, into *out.  One warp per row, atomicMax on the bit pattern (non-negative floats
+// order like their integers).  out must be zeroed first.
+__global__ void row_norm2_kernel(const float* __restrict__ x, long long N, int H, float* __restrict__ norm2,
+                                 float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
   float best = 0.0f;
@@ -139,19 +160,21 @@ __global__ void max_row_norm2_kernel(const float* __restrict__ x, long long N, i
       s = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, s))));
     }
     s = warp_sum(s);
+    if (norm2 != nullptr && lane == 0) norm2[row] = s;
     best = fmaxf(best, s);
   }
   if (lane == 0) atomicMax(reinterpret_cast<int*>(out), __float_as_int(best));
 }
 
-// per query: R = |q| * max_norm (score range), eps = TF32 error bound; zero-padded copy of the queries for the
-// scan's B operand.  One CTA per query slot (16).
+// per query: R = |q| * max_norm (score range), eps = TF32 error bound (L2: the margin of the file header, halved);
+// zero-padded copy of the queries for the scan's B operand.  One CTA per query slot (16).
 struct TcQuery {
-  float r;        // every score lies in [-r, r]
+  float r;        // every score lies in [-r, r] (L2: every v in [-r - shift, r], shift = max_norm^2 / 2)
   float eps;
   float thr;      // filled by score_threshold_kernel
   int need;       // min(k, N): rows this query must return
 };
+template <bool L2 = false>
 __global__ void tc_prepare_queries_kernel(const float* __restrict__ queries, int nq, int H, float max_norm,
                                           float* __restrict__ qpad, TcQuery* __restrict__ meta) {
   const int q = blockIdx.x;
@@ -172,6 +195,12 @@ __global__ void tc_prepare_queries_kernel(const float* __restrict__ queries, int
     const float r = sqrtf(tot) * max_norm * 1.0001f + 1e-30f;
     meta[q].r = r;
     meta[q].eps = r * (1.5f / 512.0f);
+    if constexpr (L2) {
+      const float m2 = max_norm * max_norm;
+      const float qm = sqrtf(tot) * 1.0001f + max_norm;
+      const float d = r * (1.5f / 512.0f) + static_cast<float>(H) * 0x1p-24f * m2 + 0x1p-23f * (r + m2);
+      meta[q].eps = (d + static_cast<float>(H) * 0x1p-24f * qm * qm) * 1.0001f;
+    }
     meta[q].thr = -INFINITY;
     meta[q].need = 0;
   }
@@ -185,18 +214,36 @@ __device__ __forceinline__ int tc_bin(float s, float r) {
   return b > TC_BINS - 1 ? TC_BINS - 1 : b;
 }
 
-// hist [16][TC_BINS] (zeroed before): shared-memory histograms per CTA, flushed with atomics
+// L2: the ranked value v = S - n/2 of the file header, rounded once (never contracted into an FMA, so the
+// histogram and the selection see the same bits), and its linear bin over [lo, lo + BINS / scale]
+__device__ __forceinline__ float l2_value(float s, float n2) { return __fsub_rn(s, __fmul_rn(0.5f, n2)); }
+__device__ __forceinline__ int tc_bin_l2(float v, float lo, float scale) {
+  const float u = (v - lo) * scale;
+  int b = static_cast<int>(u);
+  if (!(u > 0.0f)) b = 0;
+  return b > TC_BINS - 1 ? TC_BINS - 1 : b;
+}
+
+// hist [16][TC_BINS] (zeroed before): shared-memory histograms per CTA, flushed with atomics.  L2: of
+// v = S - norm2[row] / 2 over [-r - shift, r].
+template <bool L2 = false>
 __global__ void __launch_bounds__(512)
 score_hist_kernel(const float* __restrict__ scores, long long N, int nq, const TcQuery* __restrict__ meta,
-                  unsigned* __restrict__ hist) {
+                  unsigned* __restrict__ hist, const float* __restrict__ norm2 = nullptr, float shift = 0.0f) {
   extern __shared__ unsigned sh[];   // [nq][TC_BINS]
   for (int i = threadIdx.x; i < nq * TC_BINS; i += blockDim.x) sh[i] = 0u;
-  __shared__ float rr[TC_NQ];
-  if (threadIdx.x < TC_NQ) rr[threadIdx.x] = meta[threadIdx.x].r;
+  __shared__ float rr[TC_NQ], lo[TC_NQ];
+  if (threadIdx.x < TC_NQ) {
+    const float r = meta[threadIdx.x].r;
+    rr[threadIdx.x] = L2 ? static_cast<float>(TC_BINS) / (2.0f * r + shift) : r;
+    lo[threadIdx.x] = -r - shift;
+  }
   __syncthreads();
   for (long long row = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; row < N;
        row += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float4* p = reinterpret_cast<const float4*>(scores + static_cast<size_t>(row) * TC_NQ);
+    float n2 = 0.0f;
+    if constexpr (L2) n2 = norm2[row];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float4 v = p[i];
@@ -204,7 +251,11 @@ score_hist_kernel(const float* __restrict__ scores, long long N, int nq, const T
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int q = 4 * i + j;
-        if (q < nq) atomicAdd(&sh[q * TC_BINS + tc_bin(s[j], rr[q])], 1u);
+        if constexpr (L2) {
+          if (q < nq) atomicAdd(&sh[q * TC_BINS + tc_bin_l2(l2_value(s[j], n2), lo[q], rr[q])], 1u);
+        } else {
+          if (q < nq) atomicAdd(&sh[q * TC_BINS + tc_bin(s[j], rr[q])], 1u);
+        }
       }
     }
   }
@@ -214,8 +265,9 @@ score_hist_kernel(const float* __restrict__ scores, long long N, int nq, const T
 }
 
 // one warp per query: walk the bins from the top until `need` rows are covered
+template <bool L2 = false>
 __global__ void score_threshold_kernel(const unsigned* __restrict__ hist, int nq, long long N, int k,
-                                       TcQuery* __restrict__ meta) {
+                                       TcQuery* __restrict__ meta, float shift = 0.0f) {
   const int q = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   if (q >= nq) return;
@@ -241,30 +293,40 @@ __global__ void score_threshold_kernel(const unsigned* __restrict__ hist, int nq
   }
   if (lane == 0) {
     const float r = meta[q].r;
-    const float edge = -r + static_cast<float>(found) * (2.0f * r / static_cast<float>(TC_BINS));
-    // one extra bin width covers the rounding of the bin arithmetic itself
-    meta[q].thr = edge - 2.0f * meta[q].eps - 2.0f * r / static_cast<float>(TC_BINS);
+    if constexpr (L2) {
+      const float bin = (2.0f * r + shift) / static_cast<float>(TC_BINS);
+      meta[q].thr = (-r - shift + static_cast<float>(found) * bin) - 2.0f * meta[q].eps - bin;
+    } else {
+      const float edge = -r + static_cast<float>(found) * (2.0f * r / static_cast<float>(TC_BINS));
+      // one extra bin width covers the rounding of the bin arithmetic itself
+      meta[q].thr = edge - 2.0f * meta[q].eps - 2.0f * r / static_cast<float>(TC_BINS);
+    }
     meta[q].need = static_cast<int>(need);
   }
 }
 
-// cand [16][TC_MAX_CAND] row ids, n_cand [16] (zeroed before); counts keep growing past the cap (overflow test)
+// cand [16][TC_MAX_CAND] row ids, n_cand [16] (zeroed before); counts keep growing past the cap (overflow test).
+// L2: rows with v = S - norm2[row] / 2 >= thr.
+template <bool L2 = false>
 __global__ void __launch_bounds__(512)
 score_select_kernel(const float* __restrict__ scores, long long N, int nq, const TcQuery* __restrict__ meta,
-                    unsigned* __restrict__ cand, unsigned* __restrict__ n_cand) {
+                    unsigned* __restrict__ cand, unsigned* __restrict__ n_cand, const float* __restrict__ norm2 = nullptr) {
   __shared__ float thr[TC_NQ];
   if (threadIdx.x < TC_NQ) thr[threadIdx.x] = threadIdx.x < nq ? meta[threadIdx.x].thr : INFINITY;
   __syncthreads();
   for (long long row = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; row < N;
        row += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float4* p = reinterpret_cast<const float4*>(scores + static_cast<size_t>(row) * TC_NQ);
+    float n2 = 0.0f;
+    if constexpr (L2) n2 = norm2[row];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float4 v = p[i];
-      const float s[4] = {v.x, v.y, v.z, v.w};
+      float s[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int q = 4 * i + j;
+        if constexpr (L2) s[j] = l2_value(s[j], n2);
         if (s[j] >= thr[q]) {
           const unsigned pos = atomicAdd(&n_cand[q], 1u);
           if (pos < TC_MAX_CAND) cand[q * TC_MAX_CAND + pos] = static_cast<unsigned>(row);
@@ -276,6 +338,8 @@ score_select_kernel(const float* __restrict__ scores, long long N, int nq, const
 
 // One CTA per query: exact fp32 score of every candidate, sort (score descending, row ascending), top k out.
 // A list that overflowed or came out shorter than `need` raises *fallback (the exact scan then redoes the call).
+// L2: the score is -D, D = sum (q_i - x_i)^2 in fp32, and D is written out (ascending; a short tail is +inf / -1).
+template <bool L2 = false>
 __global__ void __launch_bounds__(512)
 exact_rescore_kernel(const unsigned* __restrict__ cand, const unsigned* __restrict__ n_cand,
                      const TcQuery* __restrict__ meta, const float* __restrict__ queries,
@@ -301,12 +365,24 @@ exact_rescore_kernel(const unsigned* __restrict__ cand, const unsigned* __restri
     const unsigned row = cand[q * TC_MAX_CAND + c];
     const float4* p = reinterpret_cast<const float4*>(corpus + static_cast<size_t>(row) * H);
     float s = 0.0f;
-    for (int i = lane; i < H / 4; i += 32) {
-      const float4 v = p[i];
-      const float4 w = *reinterpret_cast<const float4*>(qs + 4 * i);
-      s = fmaf(v.x, w.x, fmaf(v.y, w.y, fmaf(v.z, w.z, fmaf(v.w, w.w, s))));
+    if constexpr (L2) {
+      // unrolled by two: at the compiler's own choice (four) this loop spills
+#pragma unroll 2
+      for (int i = lane; i < H / 4; i += 32) {
+        const float4 v = p[i];
+        const float4 w = *reinterpret_cast<const float4*>(qs + 4 * i);
+        const float dx = w.x - v.x, dy = w.y - v.y, dz = w.z - v.z, dw = w.w - v.w;
+        s = fmaf(dx, dx, fmaf(dy, dy, fmaf(dz, dz, fmaf(dw, dw, s))));
+      }
+    } else {
+      for (int i = lane; i < H / 4; i += 32) {
+        const float4 v = p[i];
+        const float4 w = *reinterpret_cast<const float4*>(qs + 4 * i);
+        s = fmaf(v.x, w.x, fmaf(v.y, w.y, fmaf(v.z, w.z, fmaf(v.w, w.w, s))));
+      }
     }
     s = warp_sum(s);
+    if constexpr (L2) s = -s;
     if (lane == 0) {
       // order-preserving key of the float (larger score = larger key, never 0), then the inverted row id
       unsigned u = __float_as_uint(s);
@@ -342,7 +418,7 @@ exact_rescore_kernel(const unsigned* __restrict__ cand, const unsigned* __restri
       s = __uint_as_float(u);
       idx = static_cast<int64_t>(~static_cast<unsigned>(key & 0xffffffffu));
     }
-    out_score[static_cast<size_t>(q) * k + i] = s;
+    out_score[static_cast<size_t>(q) * k + i] = L2 ? -s : s;
     out_index[static_cast<size_t>(q) * k + i] = idx;
   }
 }

@@ -26,6 +26,8 @@
  *   b2e_adjacent_cosine_dist distllm/embed/embedders/semantic_chunk.py:24-55
  *   b2e_topk_ip / b2e_topk_ip_tc / b2e_max_row_norm
  *                           distllm/rag/search.py:280-336 (exact float32 search of the query path)
+ *   b2e_topk_l2 / b2e_topk_l2_tc / b2e_row_norms
+ *                           distllm/rag/search.py:402-666 (FaissIndexV1, metric='l2': faiss IndexFlatL2)
  *   b2e_gemm_h16 / b2e_attention_d64 / b2e_attention_d32 / b2e_attention_causal_d128 / b2e_qk_norm_rope /
  *   b2e_qk_layernorm_rope / b2e_layernorm:
  *                           the building blocks, exported so the parity tests can pin each kernel separately.
@@ -256,6 +258,24 @@ int b2e_topk_ip_tc(const float* queries, int Q, const float* corpus, int64_t N, 
 /* Largest Euclidean row norm of a device-resident float32 [N,H] matrix -> *out_host (synchronises `stream`:
  * an index-build step).  H % 4 == 0. */
 int b2e_max_row_norm(const float* x, int64_t N, int H, float* out_host, void* stream);
+/* Exact squared-Euclidean top-k (distllm/rag/search.py:402-666: FaissIndexV1 with metric='l2', faiss IndexFlatL2
+ * over the dataset's fp32 embeddings).  queries [Q,H] f32, corpus [N,H] F32 (row-major on the device), 1 <= k <= 256,
+ * H % 128 == 0 (zero-padded columns add (0 - 0)^2 = 0).  out_dist / out_indices are [Q,k]: D = sum_i (q_i - x_i)^2
+ * in fp32, ascending (ties: ascending index); when N < k the tail is filled with +inf / -1. */
+int b2e_topk_l2(const float* queries, int Q, const float* corpus, int64_t N, int H, int k, float* out_dist,
+                int64_t* out_indices, void* stream);
+/* The same search with the scan on the tensor cores (TF32, ranked on q.x - |x|^2 / 2) and the decision on fp32
+ * distances of the rows the approximation cannot rule out; identical contract and results (a query whose
+ * candidates do not fit the 4096-row buffer makes the call fall back to b2e_topk_l2's scan on the device).
+ * corpus_norm2 [N] f32 on the device and corpus_max_norm come from b2e_row_norms on this corpus (corpus_max_norm^2
+ * must bound every entry of corpus_norm2 and every squared row norm).  Problems below 32 768 rows go straight to
+ * b2e_topk_l2, and so do corpora of 2^31 rows or more. */
+int b2e_topk_l2_tc(const float* queries, int Q, const float* corpus, const float* corpus_norm2, int64_t N, int H,
+                   int k, float corpus_max_norm, float* out_dist, int64_t* out_indices, void* stream);
+/* Squared Euclidean norm of every row of a device-resident float32 [N,H] matrix -> out_norm2 [N] on the device
+ * (nullable; fp32, one fixed summation order), and the largest row norm (its square root) -> *out_max_host, the
+ * value b2e_max_row_norm returns.  Synchronises `stream`: an index-build step.  H % 4 == 0. */
+int b2e_row_norms(const float* x, int64_t N, int H, float* out_norm2, float* out_max_host, void* stream);
 /* Binary retrieval (distllm/rag/search.py, precision='ubinary', search_algorithm='exact'):
  * b2e_pack_ubinary = sentence_transformers quantize_embeddings(x, 'ubinary') as called from search.py:34-56
  * (np.packbits(x > 0): eight dimensions per byte, first dimension in the most significant bit), fp32

@@ -49,7 +49,8 @@ int b2e_debug_gemm_nf4_lora_rows(const void* A, const void* codes, const float* 
  * on the attended tokens only (csrc/pack.cuh).  Drops the handle's cached CUDA graphs' validity: call it before
  * b2e_embed_host, not between its batches. */
 int b2e_debug_set_packing(int on);
-/* *out = 1 when this thread's last b2e_topk_ip_tc call had to fall back to the exact scan (synchronises the device) */
+/* *out = 1 when this thread's last b2e_topk_ip_tc or b2e_topk_l2_tc call had to fall back to the exact scan
+ * (synchronises the device) */
 int b2e_debug_topk_tc_fell_back(int* out);
 /* one attention step as an encoder runs it, in the token layout it derives from the mask (csrc/pack.cuh): with
  * every mask row a non-empty prefix, qkv and ctx hold the attended tokens back to back (row cu[b] + s), else they
