@@ -107,6 +107,7 @@ DEBUG_EXPORTS = (
     'b2e_debug_attention_packed',
     'b2e_debug_rotary',
     'b2e_debug_embed',
+    'b2e_debug_roberta_positions',
     'b2e_debug_norm',
 )
 
@@ -479,6 +480,20 @@ def debug_embed(enc, input_ids: torch.Tensor, attention_mask: torch.Tensor,
         check(lib.b2e_debug_embed(enc._handle, input_ids.data_ptr(), attention_mask.data_ptr(), _ptr(token_type_ids),
                                   b, s, _ptr(out16), _ptr(xres), stream_ptr(input_ids.device)), lib)
     return out16, xres
+
+
+def debug_roberta_positions(input_ids: torch.Tensor, padding_idx: int, storage: str = 'f16') -> torch.Tensor:
+    """Debug hook: RoBERTa position ids of int64 device ids [B, S] (b2e_debug_roberta_positions) -> int32 [B, S]."""
+    lib = load(storage)
+    if _cuda_contig(input_ids, 'input_ids').dtype != torch.int64 or input_ids.dim() != 2:
+        raise NativeError('input_ids must be int64 [B, S]')
+    b, s = input_ids.shape
+    pos = torch.empty((b, s), dtype=torch.int32, device=input_ids.device)
+    lib.b2e_debug_roberta_positions.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    with torch.cuda.device(input_ids.device):
+        check(lib.b2e_debug_roberta_positions(input_ids.data_ptr(), b, s, padding_idx, pos.data_ptr(),
+                                              stream_ptr(input_ids.device)), lib)
+    return pos
 
 
 NORM_POST_LN, NORM_ADD_LN, NORM_ADD_RMS = 0, 1, 2   # b2e_debug_norm's kinds

@@ -695,6 +695,7 @@ struct B2EEncoder {
   // activations (h16); the pre-norm families' fp32 residual stream; ESM-2's token-dropout scales
   DevBuf<h16> hidden, qkv, ctx, tmp, ffn;
   DevBuf<float> xres, tok_scale;
+  DevBuf<int> pos_ids;   // [B*S] RoBERTa position rows (roberta_positions)
   PoolScratch pool;
   AttnScratch attn;
   // padding-free token layout of the pooled forward pass (pack.cuh)
@@ -744,6 +745,8 @@ struct B2EEncoder {
   }
   int ctx_cols() const { return is_decoder(desc.arch) ? desc.heads * desc.head_dim : desc.hidden; }
   bool has_xres() const { return desc.arch != B2E_ARCH_BERT; }
+  // BERT with desc.reserved = padding_idx + 1: RoBERTa / XLM-RoBERTa position ids, scanned from the input ids
+  bool roberta_positions() const { return desc.arch == B2E_ARCH_BERT && desc.reserved > 0; }
 };
 
 namespace {
@@ -767,6 +770,7 @@ int ensure_workspace(B2EEncoder* e, int B, int S) {
     return rc;
   if (e->has_xres() && (rc = e->xres.grow(tokens * H, gen, true))) return rc;
   if (e->desc.arch == B2E_ARCH_ESM2 && (rc = e->tok_scale.grow(B, gen))) return rc;
+  if (e->roberta_positions() && (rc = e->pos_ids.grow(tokens, gen))) return rc;
   if (e->lora_r128 && (rc = e->lora_u.grow(tokens * e->lora_r128, gen, true))) return rc;
   if ((rc = e->pack.ensure(B, tokens))) return rc;
   return e->pool.ensure(B, S, (size_t)B * pool_nsplit(S) * e->desc.hidden);
@@ -805,6 +809,11 @@ int validate_batch(const B2EEncoder* e, int B, int S) {
     return fail(B2E_ERR_INVALID, "encoder lives on device %d but device %d is current", e->device, cur);
   if (S > e->desc.max_pos)
     return fail(B2E_ERR_INVALID, "S=%d exceeds max_position_embeddings=%d", S, e->desc.max_pos);
+  // RoBERTa positions reach padding_idx + S: every row of the table is read in bounds, never clamped
+  const int pad = e->desc.reserved - 1;
+  if (e->roberta_positions() && S + pad >= e->desc.max_pos)
+    return fail(B2E_ERR_INVALID, "S=%d with padding_idx %d needs position rows up to %d, but the position table has "
+                "%d rows (RoBERTa positions: S <= %d)", S, pad, S + pad, e->desc.max_pos, e->desc.max_pos - pad - 1);
   return B2E_OK;
 }
 
@@ -893,12 +902,18 @@ int launch_embed(B2EEncoder* e, const int64_t* ids, const int64_t* mask, const i
   const B2EModelDesc& d = e->desc;
   const int M = B * S, H = d.hidden;
   switch (d.arch) {
-    case B2E_ARCH_BERT:   // leading slots: word, position, token-type embeddings, embedding LayerNorm g/b
+    case B2E_ARCH_BERT: {   // leading slots: word, position, token-type embeddings, embedding LayerNorm g/b
+      const int* pos_ids = nullptr;   // null: position t % S
+      if (e->roberta_positions()) {
+        roberta_positions_kernel<<<B, POS_THREADS, 0, st>>>(ids, e->pos_ids, S, d.reserved - 1);
+        pos_ids = e->pos_ids;
+      }
       DISPATCH_H(H, (embed_layernorm_kernel<HW><<<row_blocks(M), ROW_THREADS, 0, st>>>(
                          ids, types, (const float*)e->w[0], (const float*)e->w[1], (const float*)e->w[2],
                          (const float*)e->w[3], (const float*)e->w[4], hidden, M, S, d.eps, lay.t_real,
-                         lay.tok_src)));
+                         lay.tok_src, pos_ids)));
       break;
+    }
     case B2E_ARCH_ESM2: {
       const int mask_token = d.reserved - 1;  // reserved = mask_token_id + 1, 0 = token dropout off
       esm_token_scale_kernel<<<(B + 7) / 8, 256, 0, st>>>(ids, mask, e->tok_scale, B, S, mask_token);
@@ -1344,6 +1359,9 @@ int b2e_check_model(const B2EModelDesc* desc) {
       return fail(B2E_ERR_UNSUPPORTED, "ModernBERT: 2 * intermediate_size = %d must be a multiple of 256 (the gated "
                   "epilogue pairs 128 input with 128 gate columns)", 2 * desc->intermediate);
   }
+  if (desc->arch == B2E_ARCH_BERT && desc->reserved < 0)
+    return fail(B2E_ERR_INVALID, "BERT: reserved is padding_idx + 1 for RoBERTa positions or 0, got %d",
+                desc->reserved);
   if ((desc->head_dim != 64 && desc->head_dim != 32) || desc->heads * desc->head_dim != desc->hidden)
     return fail(B2E_ERR_UNSUPPORTED,
                 "need head_dim 64 or 32 and heads*head_dim == hidden (got %d heads x %d, H=%d); built: H in 256 x "
@@ -1471,7 +1489,7 @@ void b2e_encoder_destroy(B2EEncoder* e) {
   DeviceGuard guard;
   cudaSetDevice(e->device);
   for (DevBuf<h16>* b : {&e->hidden, &e->qkv, &e->ctx, &e->tmp, &e->ffn}) b->release();
-  e->xres.release(); e->tok_scale.release(); e->stage_in.release(); e->stage_out.release(); e->lora_u.release();
+  e->xres.release(); e->tok_scale.release(); e->pos_ids.release(); e->stage_in.release(); e->stage_out.release(); e->lora_u.release();
   cudaFree(e->rope_cos); cudaFree(e->rope_sin); cudaFree(e->rope_cos2); cudaFree(e->rope_sin2);
   e->pack.release();
   e->drop_graphs();
@@ -1486,6 +1504,7 @@ int64_t b2e_workspace_bytes(const B2EEncoder* e, int B, int S) {
   const size_t tokens = (size_t)B * S;
   size_t bytes = tokens_bytes(e->desc, tokens);
   if (e->has_xres()) bytes += tokens * e->desc.hidden * 4 + (size_t)B * sizeof(float);
+  if (e->roberta_positions()) bytes += tokens * sizeof(int);
   bytes += tokens * sizeof(float) + (size_t)S * sizeof(int) + (size_t)B * (2 * sizeof(int) + sizeof(float));
   bytes += (size_t)B * pool_nsplit(S) * e->desc.hidden * sizeof(float);
   bytes += tokens * e->lora_r128 * 2;
@@ -1960,9 +1979,18 @@ int b2e_debug_embed(B2EEncoder* e, const int64_t* ids, const int64_t* mask, cons
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = e->pack.ensure(B, (size_t)B * S))) return rc;
   if (arch == B2E_ARCH_ESM2 && (rc = e->tok_scale.grow(B, e->ws_gen))) return rc;
+  if (e->roberta_positions() && (rc = e->pos_ids.grow((size_t)B * S, e->ws_gen))) return rc;
   SeqLayout lay;
   if ((rc = pack_prepare(e->pack, mask, B, S, packing_enabled(), st, &lay))) return rc;
   return launch_embed(e, ids, mask, types, B, S, (h16*)out16, xres, st, lay);
+}
+
+int b2e_debug_roberta_positions(const int64_t* ids, int B, int S, int padding_idx, int* pos, void* stream) {
+  if (!ids || !pos) return fail(B2E_ERR_INVALID, "null tensor pointer");
+  if (B <= 0 || S <= 0 || padding_idx < 0) return fail(B2E_ERR_INVALID, "bad B=%d S=%d padding_idx=%d", B, S, padding_idx);
+  roberta_positions_kernel<<<B, POS_THREADS, 0, (cudaStream_t)stream>>>(ids, pos, S, padding_idx);
+  CUDA_TRY(cudaGetLastError());
+  return B2E_OK;
 }
 
 int b2e_debug_attention_packed(const void* qkv, const int64_t* mask, void* ctx, int B, int S, int heads,

@@ -119,15 +119,58 @@ __device__ __forceinline__ void warp_layernorm(float (&x)[row_passes(H)][8], con
   }
 }
 
+// RoBERTa / XLM-RoBERTa position ids (create_position_ids_from_input_ids, transformers/models/xlm_roberta/
+// modeling_xlm_roberta.py): with m = ids != pad, pos = cumsum(m) * m + pad along each sequence.  A pad id inside the
+// attended text reads row pad and does not advance the count; left padding starts the count at the first non-pad id.
+// One CTA per sequence of S ids, over chunks of POS_THREADS ids: an inclusive warp-shuffle scan of m, a scan of the 32
+// warp totals by warp 0, and the running count carried to the next chunk.  pos is [B, S], the padded layout, whatever
+// layout the embedding step then reads it in.
+constexpr int POS_THREADS = 1024;
+__global__ void __launch_bounds__(POS_THREADS)
+roberta_positions_kernel(const int64_t* __restrict__ ids, int* __restrict__ pos, int S, int pad) {
+  __shared__ int warp_total[POS_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t base = static_cast<size_t>(blockIdx.x) * S;
+  int carry = 0;
+  for (int c0 = 0; c0 < S; c0 += POS_THREADS) {
+    const int s = c0 + threadIdx.x;
+    const int m = (s < S && ids[base + s] != pad) ? 1 : 0;
+    int x = m;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_total[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      int t = warp_total[lane];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, t, o);
+        if (lane >= o) t += y;
+      }
+      warp_total[lane] = t;   // inclusive over warps 0..lane
+    }
+    __syncthreads();
+    const int count = carry + (warp > 0 ? warp_total[warp - 1] : 0) + x;
+    if (s < S) pos[base + s] = m ? count + pad : pad;
+    carry += warp_total[POS_THREADS / 32 - 1];
+    __syncthreads();   // every warp has read warp_total before the next chunk rewrites it
+  }
+}
+
 // BERT embeddings: word[ids] + position[t % S] + type[type_ids] -> LayerNorm -> h16 hidden.
 // (transformers/models/bert/modeling_bert.py:72-112)
+// pos_ids (nullable): position row of each [B,S] token (RoBERTa's rule, roberta_positions_kernel) instead of t % S.
 template <int H>
 __global__ void __launch_bounds__(ROW_THREADS)
 embed_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ type_ids,
                        const float* __restrict__ word, const float* __restrict__ pos,
                        const float* __restrict__ type, const float* __restrict__ gamma,
                        const float* __restrict__ beta, h16* __restrict__ out, int rows, int S,
-                       float eps, const int* __restrict__ n_dev, const int* __restrict__ tok_src) {
+                       float eps, const int* __restrict__ n_dev, const int* __restrict__ tok_src,
+                       const int* __restrict__ pos_ids = nullptr) {
   // n_dev / tok_src (nullable, pack.cuh): rows in use and the [B,S] position each packed row comes from
   constexpr int NV = row_passes(H);
   const int lane = threadIdx.x & 31;
@@ -137,7 +180,7 @@ embed_layernorm_kernel(const int64_t* __restrict__ ids, const int64_t* __restric
   const int src = tok_src != nullptr ? __ldg(tok_src + row) : row;
   const int64_t id = ids[src];
   const int64_t tt = type_ids ? type_ids[src] : 0;
-  const int p = src % S;
+  const int p = pos_ids != nullptr ? __ldg(pos_ids + src) : src % S;
   float x[NV][8];
 #pragma unroll
   for (int v = 0; v < NV; ++v) {

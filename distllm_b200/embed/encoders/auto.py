@@ -20,15 +20,19 @@ from distllm_b200.embed.encoders.native import NativeBertEncoder
 from distllm_b200.embed.encoders.native import NativeMistralEncoder
 from distllm_b200.embed.encoders.native import NativeModernBertEncoder
 from distllm_b200.embed.encoders.native import NativeQwen3Encoder
+from distllm_b200.embed.encoders.native import NativeRobertaEncoder
+from distllm_b200.embed.encoders.weights import roberta_max_length
 from distllm_b200.utils import BaseConfig
 
 # HF model_type -> native forward pass (BERT: post-LN encoder; Mistral: pre-RMSNorm decoder blocks
 # with rotary, grouped-query causal attention and SwiGLU, used as an encoder by the embedding models;
 # ModernBERT: pre-LN encoder with rotary, alternating full / sliding-window attention and GeGLU --
 # examples/embed/workstation/modernbert_semchunk.yaml:16-17; Qwen3: the Mistral block with a per-head RMSNorm of q
-# and k before rotary -- Qwen3-Embedding 0.6B / 4B / 8B)
+# and k before rotary -- Qwen3-Embedding 0.6B / 4B / 8B; RoBERTa / XLM-RoBERTa: the BERT block with position ids that
+# follow the padding index -- all-distilroberta-v1, BGE-M3, multilingual-e5, paraphrase-multilingual-MiniLM)
 _NATIVE_BY_MODEL_TYPE = {'bert': NativeBertEncoder, 'mistral': NativeMistralEncoder,
-                         'modernbert': NativeModernBertEncoder, 'qwen3': NativeQwen3Encoder}
+                         'modernbert': NativeModernBertEncoder, 'qwen3': NativeQwen3Encoder,
+                         'roberta': NativeRobertaEncoder, 'xlm-roberta': NativeRobertaEncoder}
 _SUPPORTED_MODEL_TYPES = tuple(_NATIVE_BY_MODEL_TYPE)
 
 
@@ -60,13 +64,17 @@ class AutoEncoderConfig(BaseConfig):
 
 
 class AutoEncoder:
-    """Encoder for HF checkpoints of the BERT, ModernBERT, Mistral and Qwen3 families on the native kernels.
+    """Encoder for HF checkpoints of the BERT, RoBERTa / XLM-RoBERTa, ModernBERT, Mistral and Qwen3 families on the
+    native kernels.
 
     Built shapes (``b2e_check_model``, checked before any weight is loaded): BERT with head_dim 64 or 32 and H in
     256 x {1,2,3,4,5,8,10,16}, 384 or 640 (all-MiniLM-L6-v2, bge-small-en-v1.5, e5-small-v2: 384 = 12 x 32);
     ModernBERT with head_dim 64 at H a multiple of 256; Mistral and Qwen3 with head_dim 128 at a built H that is a
     multiple of 256 (Qwen3-Embedding-0.6B / 4B / 8B: H = 1024 / 2560 / 4096), Qwen3 without sliding-window layers,
-    without attention biases and with default rotary."""
+    without attention biases and with default rotary.  RoBERTa and XLM-RoBERTa (model types ``roberta`` and
+    ``xlm-roberta``: all-distilroberta-v1, all-roberta-large-v1, BGE-M3, multilingual-e5-small / base / large,
+    paraphrase-multilingual-MiniLM-L12-v2) at BERT's shapes, with absolute positions, erf-GELU and ``pad_token_id``
+    set; their rows are truncated to ``max_position_embeddings - pad_token_id - 1`` tokens (512, BGE-M3: 8192)."""
 
     def __init__(self, config: AutoEncoderConfig):
         from transformers import AutoConfig
@@ -90,6 +98,12 @@ class AutoEncoder:
         )
         # proper truncation, as auto.py:74
         tokenizer.model_max_length = hf_config.max_position_embeddings
+        if _NATIVE_BY_MODEL_TYPE[hf_config.model_type] is NativeRobertaEncoder:
+            # RoBERTa positions start at padding_idx + 1, so a row of max_position_embeddings tokens would read
+            # past the table: with the reference's setting above a 513- or 514-token row (514 positions) raises
+            # IndexError in HF (a device assert on a GPU), so the reference has no output for such rows.  Truncating
+            # to the longest row the table holds only adds outputs; every row the reference embeds is unchanged.
+            tokenizer.model_max_length = roberta_max_length(hf_config)
 
         self.config = config
         state_dict = model.state_dict()

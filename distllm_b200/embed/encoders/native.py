@@ -183,6 +183,19 @@ class NativeBertEncoder:
         return out
 
 
+class NativeRobertaEncoder(NativeBertEncoder):
+    """RoBERTa and XLM-RoBERTa (``RobertaModel`` / ``XLMRobertaModel``: all-distilroberta, BGE-M3, multilingual-e5,
+    paraphrase-multilingual-MiniLM): BERT's block and weights, with position ids scanned from ``input_ids`` on the
+    device (``weights.roberta_desc``).  A batch longer than ``max_position_embeddings - pad_token_id - 1`` tokens is
+    refused: its last positions would fall outside the table."""
+
+    _DESC = staticmethod(W.roberta_desc)
+
+    def __init__(self, hf_config, *args, **kwargs) -> None:
+        super().__init__(hf_config, *args, **kwargs)
+        self.max_positions = W.roberta_max_length(hf_config)
+
+
 class NativeEsm2Encoder(NativeBertEncoder):
     """ESM-2 (pre-LayerNorm, rotary, token dropout) on the same kernels; ``token_type_ids`` unused."""
 

@@ -144,6 +144,33 @@ def bert_desc(hf_config) -> _native.ModelDesc:
     )
 
 
+def roberta_desc(hf_config) -> _native.ModelDesc:
+    """HF ``RobertaConfig`` / ``XLMRobertaConfig`` -> ``B2EModelDesc``: the BERT block and weight layout, with
+    ``reserved = pad_token_id + 1`` selecting RoBERTa's position ids (pos = cumsum(m) * m + padding_idx with
+    m = ids != padding_idx, transformers/models/xlm_roberta/modeling_xlm_roberta.py:
+    create_position_ids_from_input_ids).  The token-type table is read as in BERT, whatever its size."""
+    pos_type = getattr(hf_config, 'position_embedding_type', 'absolute')
+    if pos_type not in (None, 'absolute'):
+        raise NotImplementedError(f'position_embedding_type={pos_type!r}: only absolute position embeddings are '
+                                  f'built for RoBERTa / XLM-RoBERTa')
+    pad = getattr(hf_config, 'pad_token_id', None)
+    if pad is None or pad < 0:
+        raise NotImplementedError('RoBERTa / XLM-RoBERTa position ids follow pad_token_id, which this config does '
+                                  'not set')
+    if pad + 1 >= hf_config.max_position_embeddings:
+        raise NotImplementedError(f'pad_token_id={pad} leaves no position row of the '
+                                  f'{hf_config.max_position_embeddings}-row table for a token')
+    desc = bert_desc(hf_config)
+    desc.reserved = int(pad) + 1
+    return desc
+
+
+def roberta_max_length(hf_config) -> int:
+    """Longest row RoBERTa positions can index: its last token reads row padding_idx + S of the
+    max_position_embeddings-row table (514 -> 512, BGE-M3's 8194 -> 8192)."""
+    return hf_config.max_position_embeddings - hf_config.pad_token_id - 1
+
+
 def bert_weight_list(
     state_dict: Mapping[str, torch.Tensor],
     num_layers: int,

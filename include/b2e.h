@@ -89,7 +89,7 @@ typedef struct B2EModelDesc {
   float eps;             /* LayerNorm / RMSNorm epsilon */
   float rope_theta;      /* unused for BERT */
   int32_t sliding_window; /* Mistral: causal window (0 = none); ModernBERT: |i-j| <= sliding_window on local layers */
-  int32_t reserved;
+  int32_t reserved;       /* BERT: padding_idx + 1 selects RoBERTa / XLM-RoBERTa positions, 0 BERT's; ESM-2: see below */
   float rope_theta_local; /* ModernBERT: rotary base of the sliding-attention layers (rope_theta: full-attention layers) */
   int32_t global_every;   /* ModernBERT: layer l uses full attention iff l % global_every == 0 */
 } B2EModelDesc;
@@ -113,7 +113,11 @@ const char* b2e_last_error(void);
  * documented in distllm_b200/embed/encoders/weights.py).  Matrices
  * are of the build's 16-bit storage type (b2e_storage_dtype) [out,in] row-major, vectors and embedding
  * tables fp32.  Half values outside +-65504 saturate.  The pointers stay owned by the
- * caller and must outlive the handle.  For B2E_ARCH_ESM2, desc.reserved = mask_token_id + 1 enables
+ * caller and must outlive the handle.  For B2E_ARCH_BERT, desc.reserved = padding_idx + 1 (> 0) reads position
+ * rows as RoBERTa / XLM-RoBERTa do, from the input ids: m = ids != padding_idx, pos = cumsum(m) * m + padding_idx
+ * along each sequence (0: row t % S, BERT's); every other rule of the family is BERT's, and the encode entry points
+ * refuse S + padding_idx >= max_pos with B2E_ERR_INVALID (the last row of such a batch would read past the
+ * position table).  For B2E_ARCH_ESM2, desc.reserved = mask_token_id + 1 enables
  * ESM's token dropout rescaling (0 = off) and token_type_ids are ignored.  For B2E_ARCH_MISTRAL
  * (head_dim 128, heads % kv_heads == 0, intermediate % 128 == 0) the gate/up projection is ONE matrix
  * with rows interleaved in blocks of 64 (see B2E_EPI_SWIGLU), desc.sliding_window = 0 means none, and

@@ -72,6 +72,10 @@ int b2e_debug_rotary(struct B2EEncoder* enc, int layer, void* qkv, const int64_t
  * one a family does not write may be NULL. */
 int b2e_debug_embed(struct B2EEncoder* enc, const int64_t* ids, const int64_t* mask, const int64_t* types, int B,
                     int S, void* out16, float* xres, void* stream);
+/* RoBERTa position ids of B sequences of S input ids (the step b2e_encode runs for B2E_ARCH_BERT with
+ * desc.reserved = padding_idx + 1): m = ids != padding_idx, pos = cumsum(m) * m + padding_idx per sequence, into
+ * int32 pos [B, S].  No launch is synchronised. */
+int b2e_debug_roberta_positions(const int64_t* ids, int B, int S, int padding_idx, int* pos, void* stream);
 /* one norm step of the trunks over `rows` rows of width H, with the caller's gamma / beta, into out (out_dtype: F32 or
  * the storage type).  kind 0: LayerNorm(add + resid) over two 16-bit inputs (resid may be NULL); kind 1: xres += add
  * in the fp32 residual stream, then LayerNorm of xres; kind 2: the same with RMSNorm (beta unused).  add may be NULL
