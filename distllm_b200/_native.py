@@ -10,6 +10,7 @@ from __future__ import annotations
 import ctypes as C
 from pathlib import Path
 
+import numpy as np
 import torch
 
 # Two builds of the same sources (distllm_b200/build.py): they differ only in the 16-bit storage type of
@@ -104,6 +105,7 @@ DEBUG_EXPORTS = (
     'b2e_debug_gemm_rows',
     'b2e_debug_gemm_nf4_lora_rows',
     'b2e_debug_topk_tc_fell_back',
+    'b2e_debug_topk_tc_state',
     'b2e_debug_attention_packed',
     'b2e_debug_rotary',
     'b2e_debug_embed',
@@ -659,6 +661,22 @@ def topk_tc_fell_back() -> bool:
     lib.b2e_debug_topk_tc_fell_back.argtypes = [C.POINTER(C.c_int)]
     check(lib.b2e_debug_topk_tc_fell_back(C.byref(out)))
     return bool(out.value)
+
+
+TC_QUERY_DTYPE = np.dtype([('r', '<f4'), ('eps', '<f4'), ('thr', '<f4'), ('need', '<i4')])
+
+
+def topk_tc_state(rows: int) -> dict[str, np.ndarray]:
+    """The intermediate state of the last pass (<= 16 queries) of this thread's last tensor-core search (debug
+    hook): 'scores' [rows, 16] f32 (the TF32 scan), 'meta' [16] records (r, eps, thr, need), 'hist' [16, 2048],
+    'cand' [16, 4096] row ids and 'n_cand' [16], all uint32 but the first two.  Synchronises the device."""
+    lib = load()
+    out = {'scores': np.empty((rows, 16), np.float32), 'meta': np.empty(16, TC_QUERY_DTYPE),
+           'hist': np.empty((16, 2048), np.uint32), 'cand': np.empty((16, 4096), np.uint32),
+           'n_cand': np.empty(16, np.uint32)}
+    lib.b2e_debug_topk_tc_state.argtypes = [C.c_int64] + [C.c_void_p] * 5
+    check(lib.b2e_debug_topk_tc_state(rows, *(a.ctypes.data for a in out.values())), lib)
+    return out
 
 
 def pack_ubinary(embeddings: torch.Tensor) -> torch.Tensor:

@@ -2246,6 +2246,25 @@ int b2e_debug_topk_tc_fell_back(int* out) {
   return B2E_OK;
 }
 
+// copies of the last pass's scan scores, query records, histograms and candidate lists (synchronises the device)
+int b2e_debug_topk_tc_state(int64_t rows, float* scores, void* meta, uint32_t* hist, uint32_t* cand,
+                            uint32_t* n_cand) {
+  static_assert(sizeof(TcQuery) == 16, "b2e_debug.h documents a 16-byte record");
+  TcScratch& sc = g_tc_scratch;
+  if (sc.meta.p == nullptr) return fail(B2E_ERR_INVALID, "topk_tc_state: no tensor-core search ran on this thread");
+  if (rows < 0 || (size_t)rows * TC_NQ > sc.scores.cap)
+    return fail(B2E_ERR_INVALID, "topk_tc_state: rows=%lld, the score buffer holds %zu", (long long)rows,
+                sc.scores.cap / TC_NQ);
+  CUDA_TRY(cudaDeviceSynchronize());
+  if (scores) CUDA_TRY(cudaMemcpy(scores, sc.scores, (size_t)rows * TC_NQ * sizeof(float), cudaMemcpyDeviceToHost));
+  if (meta) CUDA_TRY(cudaMemcpy(meta, sc.meta, TC_NQ * sizeof(TcQuery), cudaMemcpyDeviceToHost));
+  if (hist) CUDA_TRY(cudaMemcpy(hist, sc.hist, (size_t)TC_NQ * TC_BINS * sizeof(unsigned), cudaMemcpyDeviceToHost));
+  if (cand)
+    CUDA_TRY(cudaMemcpy(cand, sc.cand, (size_t)TC_NQ * TC_MAX_CAND * sizeof(unsigned), cudaMemcpyDeviceToHost));
+  if (n_cand) CUDA_TRY(cudaMemcpy(n_cand, sc.n_cand, TC_NQ * sizeof(unsigned), cudaMemcpyDeviceToHost));
+  return B2E_OK;
+}
+
 // ---- ubinary retrieval: packed bits, Hamming top-K, float rescoring (binsearch.cuh)
 extern "C++" {
 namespace {

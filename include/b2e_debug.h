@@ -52,6 +52,13 @@ int b2e_debug_set_packing(int on);
 /* *out = 1 when this thread's last b2e_topk_ip_tc or b2e_topk_l2_tc call had to fall back to the exact scan
  * (synchronises the device) */
 int b2e_debug_topk_tc_fell_back(int* out);
+/* the intermediate state of the last pass (its <= 16 queries) of this thread's last b2e_topk_ip_tc or
+ * b2e_topk_l2_tc call that took the tensor-core path, copied into host buffers; each may be NULL.  scores [rows, 16]
+ * f32 (the TF32 scan: row n, query q at n * 16 + q; rows at most N rounded up to 128), meta [16] records of 16 bytes
+ * {float r, eps, thr; int32 need}, hist [16, 2048], cand [16, 4096] row ids, n_cand [16] (counts past 4096 mean the
+ * list overflowed).  Synchronises the device; launches nothing. */
+int b2e_debug_topk_tc_state(int64_t rows, float* scores, void* meta, uint32_t* hist, uint32_t* cand,
+                            uint32_t* n_cand);
 /* one attention step as an encoder runs it, in the token layout it derives from the mask (csrc/pack.cuh): with
  * every mask row a non-empty prefix, qkv and ctx hold the attended tokens back to back (row cu[b] + s), else they
  * are [B*S] rows in the padded layout.  Both span B*S rows.  causal = 0: bidirectional, head_dim 32 or 64
