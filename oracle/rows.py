@@ -247,6 +247,164 @@ def l2_exact(x: np.ndarray) -> np.ndarray:
     return x / np.maximum(np.sqrt(ss), L2_EPS)[:, None]
 
 
+# ------------------------------------------------------------------------------------------- ESM C
+# ESM C's widths are not 2^k * {1, 3, 5}: 960 = 15 x 64 and 1152 = 9 x 128, the odd factor's signs the Kronecker
+# product of two of ODD_SIGNS' rows.  Rows are 2^6 * pattern: var + eps rounds to 4^6 at both widths for eps 1e-12 and
+# 1e-5, fused or not (2^5 is not enough at 960 with eps 1e-5; tests/test_esmc_exact_cpu.py).
+ODD = {960: (3, 5), 1152: (3, 3)}
+ESMC_SCALE = 6
+ESMC_HEAD = 64
+
+
+def esmc_pattern(h: int, k: int) -> np.ndarray:
+    a, b = ODD[h]
+    n = h // (a * b)
+    return np.kron(np.kron(ODD_SIGNS[a], ODD_SIGNS[b]), walsh(n, k))
+
+
+def esmc_order(h: int) -> int:
+    """n, the Walsh order of an ESM C width."""
+    return h // (ODD[h][0] * ODD[h][1])
+
+
+def esmc_walsh_rows(count: int, h: int, a: int = ESMC_SCALE) -> np.ndarray:
+    """[count, h]: row i = 2^a * sign_i * esmc_pattern(h, index_i), distinct for i < n - 2 (as walsh_rows)."""
+    m = esmc_order(h) // 2 - 1
+    return np.stack([(1.0 if (i // m) % 2 == 0 else -1.0) * 2.0 ** a * esmc_pattern(h, 1 + i % m)
+                     for i in range(count)])
+
+
+def esmc_gain(h: int, j: int, sign: float = 1.0) -> np.ndarray:
+    return sign * 2.0 ** j * esmc_pattern(h, esmc_order(h) // 2)
+
+
+def qk_gains(h: int, which: int) -> np.ndarray:
+    """q_ln (which 0) or k_ln (1) gains of ESM C's fused q / k step: signed powers of two 2^-3 .. 2^3 whose exponent
+    changes between q and k, between the two halves of a head (c, c + 32) and between heads (c, c + 64) -- a swapped
+    gain, a wrong partner or a wrong head changes the bits -- and a few zeros, whose partners' outputs are then the
+    table entries alone."""
+    c = np.arange(h)
+    e = (5 * c + 3 * (c // ESMC_HEAD) + 2 * (c % ESMC_HEAD >= 32) + 4 * which) % 7 - 3
+    sign = np.where(((3 * c + c // ESMC_HEAD + which) // 2) % 2 == 0, 1.0, -1.0)
+    g = sign * 2.0 ** e
+    g[(c + 13 * which) % 37 == 5] = 0.0
+    return g
+
+
+def rope_exact(y, cos, sin, pos) -> np.ndarray:
+    """The halves rotation of fp32 rows y [T, W] (64-wide heads) at positions pos with the fp32 tables cos / sin
+    [S, 32], for rows whose every product with the table is exact in fp32 (powers of two, 0): round32(y1 c - y2 s),
+    round32(y2 c + y1 s) -- one rounding, whether or not the products are contracted into fmas.  float32 [T, W]."""
+    y = np.asarray(y, np.float32)
+    t, w = y.shape
+    y = y.reshape(t, w // ESMC_HEAD, 2, ESMC_HEAD // 2)
+    c = np.asarray(cos, np.float32)[pos][:, None, :]
+    s = np.asarray(sin, np.float32)[pos][:, None, :]
+    y1, y2 = y[:, :, 0], y[:, :, 1]
+    p2s, p1s = y2 * s, y1 * s
+    for a, b, p in ((y2, s, p2s), (y1, s, p1s)):
+        if not np.array_equal(p.astype(np.float64), a.astype(np.float64) * b.astype(np.float64)):
+            raise ValueError('a product of the rotation is not exact in fp32')
+    return np.stack([fma32(y1, c, -p2s), fma32(y2, c, p1s)], 2).reshape(t, w)
+
+
+def rotary_table(pos, base: float = 10000.0, d: int = ESMC_HEAD):
+    """The fp32 rotary table of HF's rotary embeddings and of esm's (esm/layers/rotary.py of the esm package),
+    restated from their documented behaviour: inv_freq = 1 / base^(arange(0, d, 2) / d) in fp32, the angle the fp32
+    product position * inv_freq, then cos and sin.  Returns float64 (cos, sin, tau) [len(pos), d/2]: tau allows the
+    device's table 8 fp32 ulps of the angle plus 8 of the result (tests/test_gpu_rows_exact.py's rotary_reference
+    uses it too)."""
+    inv = 1.0 / (torch.tensor(base, dtype=torch.float32) ** (torch.arange(0, d, 2).float() / d))
+    ang = (torch.from_numpy(np.asarray(pos, np.float32))[:, None] * inv[None]).double().numpy()
+    return np.cos(ang), np.sin(ang), np.abs(ang) * 2.0 ** -20 + 2.0 ** -21
+
+
+def warp_butterfly(v: np.ndarray) -> np.ndarray:
+    """warp_sum over the last axis (32 lanes) in fp32: v += shfl_xor(v, o) for o = 16 .. 1."""
+    lane = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        v = (v + v[..., lane ^ o]).astype(np.float32)
+    return v[..., 0]
+
+
+def qk_layernorm_rope_fp32(x, gamma, cos, sin, pos, eps: float) -> np.ndarray:
+    """qk_layernorm_rope_kernel's fp32 arithmetic on one side (the q or the k rows x [T, H]) restated on the host:
+    each lane's sum over its columns in pass order, the warp butterfly, mean = fl(sum * fl(1/H)); fmaf sums of
+    squares of x - mean over the on lanes, var = fma(ss, fl(1/H), eps), rstd correctly rounded (rsqrtf is within 2
+    ulp), y = fl(fl((x - mean) rstd) g); the rotation with contracted products.  float32 [T, H]."""
+    x = np.asarray(x, np.float32)
+    t, h = x.shape
+    nv = (h + 255) // 256
+    pad = np.zeros((t, nv * 256), np.float32)
+    pad[:, :h] = x
+    lanes = pad.reshape(t, nv, 32, 8).transpose(0, 2, 1, 3).reshape(t, 32, nv * 8)
+    on = np.zeros(nv * 256, bool)
+    on[:h] = True
+    on = on.reshape(nv, 32, 8).transpose(1, 0, 2).reshape(32, nv * 8)
+    inv_h = np.float32(1) / np.float32(h)
+    s = np.zeros((t, 32), np.float32)
+    for k in range(nv * 8):
+        s = (s + lanes[:, :, k]).astype(np.float32)
+    mean = (warp_butterfly(s) * inv_h).astype(np.float32)[:, None, None]
+    d = (lanes - mean).astype(np.float32)
+    ss = np.zeros((t, 32), np.float32)
+    for k in range(nv * 8):
+        ss = np.where(on[:, k], fma32(d[:, :, k], d[:, :, k], ss), ss)
+    var = fma32(warp_butterfly(ss), inv_h, np.float32(eps))
+    rstd = (1.0 / np.sqrt(var.astype(np.float64))).astype(np.float32)[:, None, None]
+    y = (d * rstd).astype(np.float32)
+    y = y.reshape(t, 32, nv, 8).transpose(0, 2, 1, 3).reshape(t, nv * 256)[:, :h]
+    y = (y * np.asarray(gamma, np.float32)).astype(np.float32).reshape(t, h // ESMC_HEAD, 2, ESMC_HEAD // 2)
+    c = np.asarray(cos, np.float32)[pos][:, None, :]
+    sn = np.asarray(sin, np.float32)[pos][:, None, :]
+    y1, y2 = y[:, :, 0], y[:, :, 1]
+    return np.stack([fma32(y1, c, -(y2 * sn)), fma32(y2, c, y1 * sn)], 2).reshape(t, h)
+
+
+def qk_layernorm_rope_bound(x, gamma, cos, sin, pos, eps: float):
+    """(reference, bound) of ESM C's q / k step on one side, rows x [T, H] of 16-bit values: the float64 LayerNorm
+    without bias, gain, and the rotation with the fp32 table values handed to the kernel.  Any fp32 evaluation of the
+    kernel's steps is within bound of the reference before its one 16-bit rounding, u = 2^-24:
+      the mean      |dmu| <= (H + 2) u mean|x|   (a sum of H terms, the product with fl(1/H))
+      the scale     relative (H + 16) u / 2 + (dmu / sigma)^2   (var: a sum of H positive squares, fl(1/H) and the
+                    product with it, + eps: (H + 2) u, halved by the square root; rsqrtf's 2 ulps: 4u; x - mean and
+                    the two products of y: 3u; the mean's error adds (dmu / sigma)^2 to var)
+      so            |dy| <= |g| rstd (dmu + |x - mu| scale)
+      the rotation  |c| |dy1| + |s| |dy2| plus one rounding per product and one per sum: 2u (|y1 c| + |y2 s|)."""
+    x = np.asarray(x, np.float64)
+    t, h = x.shape
+    u = 2.0 ** -24
+    mu = x.mean(-1, keepdims=True)
+    d = x - mu
+    var = (d * d).mean(-1, keepdims=True) + np.float32(eps)
+    r = 1.0 / np.sqrt(var)
+    dmu = (h + 2) * u * np.abs(x).mean(-1, keepdims=True)
+    scale = (h + 16) * u / 2 + dmu * dmu / var
+    g = np.asarray(gamma, np.float64)
+    y = (d * r * g).reshape(t, h // ESMC_HEAD, 2, ESMC_HEAD // 2)
+    dy = (np.abs(g) * r * (dmu + np.abs(d) * scale)).reshape(y.shape)
+    c = np.asarray(cos, np.float32)[pos][:, None, :].astype(np.float64)
+    s = np.asarray(sin, np.float32)[pos][:, None, :].astype(np.float64)
+    y1, y2, d1, d2 = y[:, :, 0], y[:, :, 1], dy[:, :, 0], dy[:, :, 1]
+    ref = np.stack([y1 * c - y2 * s, y2 * c + y1 * s], 2).reshape(t, h)
+    b1 = np.abs(c) * d1 + np.abs(s) * d2 + 2 * u * (np.abs(y1 * c) + np.abs(y2 * s))
+    b2 = np.abs(c) * d2 + np.abs(s) * d1 + 2 * u * (np.abs(y2 * c) + np.abs(y1 * s))
+    return ref, np.stack([b1, b2], 2).reshape(t, h) * (1 + 2.0 ** -10)
+
+
+def interval_check(got, ref, bound, dtype) -> str | None:
+    """got = round16(v) for some v within bound of ref: got in [round16(ref - bound), round16(ref + bound)] (rounding
+    is monotonic).  None, or a description of the first element outside."""
+    got = np.asarray(got, np.float64)
+    lo, hi = round16(ref - bound, dtype), round16(ref + bound, dtype)
+    bad = ~((got >= lo) & (got <= hi))
+    if not bad.any():
+        return None
+    i = tuple(int(k) for k in np.argwhere(bad)[0])
+    return (f'{bad.sum()} of {bad.size} outside; first at {i}: got {got[i]!r}, reference {ref[i]!r} '
+            f'+- {bound[i]:.3g}')
+
+
 # ------------------------------------------------------------------------------------------- row-path encoders
 # Every weight matrix zero: by the GEMM's bias provenance every linear layer outputs exactly round16(bias), and
 # attention is multiplied by a zero matrix.  What remains of each family's forward pass is its row kernels:
@@ -254,7 +412,10 @@ def l2_exact(x: np.ndarray) -> np.ndarray:
 #   ESM-2       xres = word * mask, += round16(bo_l), += round16(b2_l) in that order; final LN(xres)
 #   ModernBERT  xres = LN_emb(tok) (no biases anywhere); final LN(xres)
 #   Mistral / Qwen3   xres = embed; final RMSNorm(xres)
-# The inner pre-norm LayerNorms of ESM-2, ModernBERT and the decoders feed zero matrices only.
+#   ESM C       xres = embed; final LN(xres) without bias (the pre-norm LayerNorms carry biases, but feed zero
+#               matrices only, and no Linear layer has a bias).  Its q / k rows are exactly 0, and the
+#               fused q / k LayerNorm maps them to (0 - 0) * rsqrt(eps) * gain = 0 (NaN without eps)
+# The inner pre-norm LayerNorms of ESM-2, ModernBERT, ESM C and the decoders feed zero matrices only.
 VOCAB = 48
 LAYERS = 2
 ESM_BIASES = (2.0 ** 15, 2.0 ** 14, 2.0 ** 14, -2.0 ** 15)   # bo0, b20, bo1, b21: xres reaches 2^16 +- 32
@@ -273,6 +434,19 @@ def row_path_model(fam: str, h: int, live: str = 'word', max_pos: int = 1100):
     kernels.  ``reference(ids, mask, types)`` -> float64 [B, S, H] final hidden state, exact fp32 values.
     BERT: ``live`` names the one embedding table ('word', 'pos', 'type') that holds Walsh rows; the others are 0."""
     from distllm_b200.embed.encoders import weights as W
+
+    if fam == 'esmc':
+        sd = _zero_matrices(W.random_esmc_state_dict(h, LAYERS, 256, seed=h, vocab=VOCAB))
+        emb = esmc_walsh_rows(VOCAB, h)
+        emb[VOCAB - 1] = 0.0          # the final LayerNorm of a zero row: 0, and NaN without eps
+        sd['embed.weight'] = _t(emb)
+        g_f = esmc_gain(h, 3, -1.0)
+        sd['transformer.norm.weight'] = _t(g_f)
+        cfg = W.esmc_config(sd)
+
+        def reference(ids, mask, types, dtype):
+            return layernorm(emb[ids.numpy()], g_f, 0.0, W.ESMC_EPS)
+        return cfg, sd, reference
 
     n, _ = split_width(h)
     beta_f = 2.0 ** 3 * pattern(h, 1 + (n // 2 - 2) % (n // 2 - 1))     # the final norm's bias: a pattern
@@ -394,4 +568,5 @@ def row_path_model(fam: str, h: int, live: str = 'word', max_pos: int = 1100):
 FAMILY_WIDTHS = {'bert': WIDTHS, 'esm': WIDTHS,
                  'modernbert': tuple(h for h in WIDTHS if h % 256 == 0),
                  'mistral': tuple(h for h in WIDTHS if h % 256 == 0),
-                 'qwen3': tuple(h for h in WIDTHS if h % 256 == 0)}
+                 'qwen3': tuple(h for h in WIDTHS if h % 256 == 0),
+                 'esmc': tuple(ODD)}

@@ -45,6 +45,9 @@ INSTANTIATIONS = {
     **{f'd64-v{v}': (64, 0, v, 2, 2) for v in (0, 1, 5, 64, 65, 69, 193)},
     **{f'win-v{v}': (64, 1, v, 2, 2) for v in (0, 64, 128, 192)},
     **{f'gqa{r}': (128, 2, None, 4, 4 // r) for r in (1, 2, 4)},
+    # ESM C's head counts (esmc-300m, esmc-600m): qkv rows of 2880 and 3456 columns
+    'esmc15': (64, 0, None, 15, 15),
+    'esmc18': (64, 0, None, 18, 18),
 }
 RAGGED = (513, 512, 511, 257, 256, 255, 129, 128, 127, 65, 64, 63, 1)
 # shape: (S, lengths of the right-padded rows or a named mask, rows of K scaled up along the sequence, q scale)

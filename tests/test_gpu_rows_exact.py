@@ -175,10 +175,7 @@ def rotary_reference(x: np.ndarray, pos: np.ndarray, theta: float, d: int, gamma
     product each) plus 8 of the result (sincosf, torch's cos); the rotation adds one rounding per product and one per
     sum (2^-23 of |x1| + |x2|), Qwen3's norm 2^-20 relative (rsqrtf, three products)."""
     half = d // 2
-    inv = 1.0 / (torch.tensor(theta, dtype=torch.float32) ** (torch.arange(0, d, 2).float() / d))
-    ang = (torch.from_numpy(pos.astype(np.float32))[:, None] * inv[None]).double().numpy()     # fl32 products
-    c, s = np.cos(ang)[:, None, :], np.sin(ang)[:, None, :]
-    tau = (np.abs(ang) * 2.0 ** -20 + 2.0 ** -21)[:, None, :]
+    c, s, tau = (a[:, None, :] for a in R.rotary_table(pos, theta, d))
     rel = 2.0 ** -23
     if gamma is not None:
         r = 1.0 / np.sqrt((x * x).mean(-1, keepdims=True) + np.float32(eps))
@@ -194,13 +191,8 @@ def rotary_check(got: np.ndarray, ref: np.ndarray, bound: np.ndarray, dtype) -> 
     """got = round16(v) for some v within bound of ref: got in [round16(ref - bound), round16(ref + bound)]
     (rounding is monotonic), so one 16-bit ulp away from round16(ref) only where the bound straddles a rounding
     boundary."""
-    lo, hi = R.round16(ref - bound, dtype), R.round16(ref + bound, dtype)
-    bad = ~((got >= lo) & (got <= hi))
-    if not bad.any():
-        return None
-    i = tuple(int(k) for k in np.argwhere(bad)[0])
-    return (f'{bad.sum()} of {bad.size} outside; first at row {i[0]}, head {i[1]}, element {i[2]}: '
-            f'got {got[i]!r}, reference {ref[i]!r} +- {bound[i]:.3g}')
+    msg = R.interval_check(got, ref, bound, dtype)
+    return None if msg is None else msg + ' (index: row, head, element)'
 
 
 def rotary_masks():
@@ -358,7 +350,8 @@ def masks(s: int) -> dict[str, torch.Tensor]:
     return out
 
 
-# full mask set and S values at the widths with a half pass and at the BERT-base width, S = 129 elsewhere
+# full mask set and S values at the widths with a half pass, at the BERT-base width and for ESM C (whose widths both end
+# on a partial pass), S = 129 elsewhere
 FULL_WIDTHS = (384, 640, 768)
 SEQS = (1, 64, 65, 129, 1100)
 
@@ -399,15 +392,16 @@ def test_row_path_encoder_exact(dev, fam, h, live, storage):
     from distllm_b200.embed.encoders import native as N
 
     cls = {'bert': N.NativeBertEncoder, 'esm': N.NativeEsm2Encoder, 'modernbert': N.NativeModernBertEncoder,
-           'mistral': N.NativeMistralEncoder, 'qwen3': N.NativeQwen3Encoder}[fam]
+           'mistral': N.NativeMistralEncoder, 'qwen3': N.NativeQwen3Encoder, 'esmc': N.NativeEsmcEncoder}[fam]
     cfg, sd, reference = R.row_path_model(fam, h, live)
     dtype = nv.STORAGE_TORCH_DTYPE[storage]
     enc = cls(cfg, sd, device=dev, storage=storage)
-    seqs = SEQS if h in FULL_WIDTHS else (65, 129)
+    full = h in FULL_WIDTHS or fam == 'esmc'
+    seqs = SEQS if full else (65, 129)
     try:
         for s in seqs:
             for mname, mask in masks(s).items():
-                if h not in FULL_WIDTHS and s == 65 and mname != 'holes':
+                if not full and s == 65 and mname != 'holes':
                     continue
                 ids, types = make_inputs(fam, live, mask, seed=h + s)
                 y = reference(ids, mask, types, dtype)
